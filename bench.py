@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — audio-seconds per wall-second of the Whisper hot path on B200 (BASELINE.json metric).
+"""bench.py — audio-seconds per wall-second of the Whisper hot path on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]                  # this engine
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   # this engine
     python bench.py --impl reference [--gpus N] [--steps K] [--warmup W] # the reference's own CPU path on the host cores
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...   # N > 1, one rank per GPU
 
@@ -14,9 +14,14 @@ reference thread count the decoder reproduces), and the line says whether the to
   value : whole-job audio-s/s with the PCM already resident in HBM (wsp_upload_pcm + wsp_run_chunks_resident) — the log-mel
           front end, encoder and decoder all run inside the timed region; device time from CUDA events on the launching stream.
   e2e   : the same through the public C-ABI call with HOST buffers (wsp_run_chunks): pinned PCM -> H2D every step, tokens D2H.
-  roofline: the dominant kernel (decode_flow_kernel: the single-launch dataflow decoder step) against the
-          measured HBM peak; its per-launch duration is measured live by an instrumented decoder pass (CUDA event pair around every launch).
+  roofline: the dominant kernel (decode_flow_kernel: the single-launch dataflow decoder step) against the HBM peak
+          (MEASURED_PEAKS.json when present, else the H100 SXM data sheet's 3.35 TB/s); its per-launch duration is measured live by an
+          instrumented decoder pass (CUDA event pair around every launch).
   cpu_baseline: oracle/_ref (the reference's unmodified ggml.c + whisper.cpp) on this box's host cores, bounded sample.
+
+--dump-outputs DIR: after the timed steps, rank 0 writes what the last timed step returned — tokens.npy ([batch, n_decode] token ids
+as float64) and last_logits.npy ([batch, n_vocab] float32 logits of the final decoder step).  Inputs are seeded, so two builds run with
+the same arguments can be compared output for output.
 
 Multi-GPU: chunks are independent, so ranks shard the batch with no data-path collective ("weak" scaling: batch per GPU fixed).
 The only collective is the NCCL broadcast of the ggml file image at load (rank 0 reads the file once).
@@ -38,7 +43,7 @@ if ROOT not in sys.path:
 
 import numpy as np  # noqa: E402
 
-METRIC = "audio-sec/s (RTF) medium 30s chunks @1/2/4/8 B200 vs reference CPU path"
+METRIC = "audio-sec/s (RTF) medium 30s chunks @1/2/4/8 H100 vs reference CPU path"
 UNIT = "audio-s/s"
 CHUNK_SECONDS = 30.0
 
@@ -60,6 +65,7 @@ def parse_args():
     ap.add_argument("--chunk-base", type=int, default=-1, help="debug: use synthetic chunks base .. base+B-1 instead of the fixture's (no token check)")
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the reference CPU leg (model sweeps; the default run keeps it)")
     ap.add_argument("--ref-tokens", type=int, default=12, help="reference arm: decoder tokens actually run per sample")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs to DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -79,7 +85,7 @@ def hbm_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (not measured)"
 
 
 def _jsonable(o):
@@ -295,7 +301,7 @@ def _run_ours(a, real_stdout):
             # EVERY rank runs the chunks of the pinned configuration and is checked against the fixture (replicas: the chunks of
             # different GPUs are independent either way).  Chunks outside the calibrated family can throw the scripted decoder off its
             # script into rows whose top probability is shared, and every such row costs the sampler its exact std::partial_sort
-            # emulation (~110 us, one thread): measured 109 instead of 97 ms per 100 tokens on chunk ids 72..79
+            # emulation
             chunk_ids = [int(x) for x in fx[key + "_chunks"]]
             fixture_tokens = fx[pre + "_tokens"] if pre + "_tokens" in fx else None
     except Exception:
@@ -380,6 +386,11 @@ def _run_ours(a, real_stdout):
         per_rank = [{"rank": i, "ms_per_step": float(t[0]), "mel_ms": float(t[1]), "encode_ms": float(t[2]), "decode_ms": float(t[3]), "sm_mhz": float(t[4])}
                     for i, t in enumerate(allr)]
     same_tokens = bool((toks_r == toks).all())
+    if a.dump_outputs and rank == 0:
+        # what the last timed step returned; read back before the instrumented decoder pass below overwrites the logits
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        np.save(os.path.join(a.dump_outputs, "tokens.npy"), np.asarray(toks_r, np.float64))
+        np.save(os.path.join(a.dump_outputs, "last_logits.npy"), np.asarray(ctx.logits(B), np.float32))
 
     # ---- roofline of the dominant kernel: instrumented decoder pass (event pair around every launch) ----
     n_prof = 6
@@ -404,18 +415,8 @@ def _run_ours(a, real_stdout):
         kernel = "kern::skinny_gemm_kernel (decoder weight-streaming GEMM, 6 per layer + logits)"
         detail = {"launches_per_decoder_step": per_step}
     achieved = bytes_per_launch / (ms_per_launch * 1e-3) / 1e9
-    # measured DRAM traffic of that kernel (ncu --set full, one capture per kernel change): profiles/ncu_traffic.json
-    traffic = None
-    if per_step <= 1.5:
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-            ent = tj.get("decode_flow_kernel<%d>|B=%d|L=%d|T=%d" % (model.n_text_state, B, model.n_text_layer, model.n_audio_ctx))
-            if ent:
-                traffic = ent["dram_bytes_per_launch"]
-        except Exception:
-            traffic = None
     roofline = {
-        "kernel": kernel, "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+        "kernel": kernel, "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
         "peak_source": peak_src, "bytes_per_launch": bytes_per_launch, "ms_per_launch": ms_per_launch,
         "decoder_step_ms_by_kind": {"decoder_kernel": ms_kind[0] / n_prof, "cross_attention": ms_kind[1] / n_prof, "self_attention": ms_kind[2] / n_prof, "sampler": ms_kind[3] / n_prof},
         "how": "wsp_profile_decode: %d un-graphed decoder steps, cudaEvent pair around every launch on the launching stream" % n_prof,

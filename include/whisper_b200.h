@@ -1,4 +1,4 @@
-/* whisper_b200 — C ABI of the B200-native Whisper hot path.
+/* whisper_b200 — C ABI of the H100-native Whisper hot path.
  *
  * This is the thin extern-"C" layer BASELINE.json's north_star asks for: plain pointers and sizes, no C++ or torch types.
  * The COM-style iModel / iContext shells of the reference (include/whisper_b200_com.h) sit on top of it, exactly where the
@@ -20,7 +20,7 @@
  *
  * Error handling mirrors the reference's HRESULT convention (SURVEY.md §8b): every function returns a wsp_status that the COM
  * shell maps 1:1 to an HRESULT; no exception crosses this boundary.  There is NO CPU fallback: if the CUDA device or the
- * sm_100a kernels are unavailable the calls fail with WSP_E_CUDA.
+ * sm_90a kernels are unavailable the calls fail with WSP_E_CUDA.
  *
  * Threading: a wsp_model / wsp_engine is immutable after creation and may be shared; a wsp_context is single-threaded state
  * (KV memories, workspaces), one per concurrent stream — the same contract as iModel / iContext (Whisper/Whisper/WhisperModel.h:28-31).
@@ -43,7 +43,7 @@ enum
 	WSP_E_POINTER = -2,
 	WSP_E_FILE = -3,          /* cannot open / truncated */
 	WSP_E_FORMAT = -4,        /* not a ggml whisper file, missing or mis-shaped tensors */
-	WSP_E_CUDA = -5,          /* CUDA runtime / driver failure, or no sm_100a device */
+	WSP_E_CUDA = -5,          /* CUDA runtime / driver failure, or no sm_90a device */
 	WSP_E_OUTOFMEMORY = -6,
 	WSP_E_BOUNDS = -7,        /* batch, token count or context length beyond what the context was created for */
 	WSP_E_NOTIMPL = -8,
@@ -200,7 +200,7 @@ void wsp_host_free( void* p );
 wsp_status wsp_timings( wsp_context* c, float ms4[ 4 ], int32_t calls4[ 4 ], int32_t reset );
 
 /* ---- kernel-level test hooks (tests/ only) ---- */
-/* D[M][N] = A[M][K] * B[N][K]^T with the tcgen05 GEMM; A,B f16 bit patterns (uint16), D f32; all host pointers */
+/* D[M][N] = A[M][K] * B[N][K]^T with the wgmma GEMM; A,B f16 bit patterns (uint16), D f32; all host pointers */
 wsp_status wsp_test_gemm( int32_t device, int32_t M, int32_t N, int32_t K, const uint16_t* A, const uint16_t* B, float* D, int32_t bn, int32_t iters, float* ms );
 /* encoder attention: Q,K [BH][T][64], V [BH][T][64] f16 bit patterns -> out f32 [BH][T][64] */
 wsp_status wsp_test_attention( int32_t device, int32_t BH, int32_t T, const uint16_t* Q, const uint16_t* K, const uint16_t* V, float* out, int32_t iters, float* ms );

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (sm_100a) and the built libwhisper_b200.so")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a) and the built libwhisper_b200.so")
 
 
 def _has_gpu():

@@ -1,5 +1,5 @@
 """C-ABI surface: the shared library loads, exports every symbol include/whisper_b200.h declares, parses model files on the
-host, and FAILS LOUDLY (no CPU fallback) when asked to compute without an sm_100a device.  No GPU needed."""
+host, and FAILS LOUDLY (no CPU fallback) when asked to compute without an sm_90a device.  No GPU needed."""
 import os
 import re
 
@@ -29,7 +29,7 @@ def test_library_exports_every_declared_symbol():
 
 def test_version_and_error_text():
     L = capi.lib()
-    assert b"sm_100a" in L.wsp_version()
+    assert b"sm_90a" in L.wsp_version()
     assert isinstance(L.wsp_last_error(), bytes)
 
 
@@ -86,7 +86,7 @@ def test_meta_blob_roundtrip():
 
 
 def test_no_cpu_fallback_without_gpu():
-    """On a box without a B200 every compute entry point must fail with WSP_E_CUDA and say why."""
+    """On a box without an H100 every compute entry point must fail with WSP_E_CUDA and say why."""
     L = capi.lib()
     if L.wsp_device_count() > 0:
         pytest.skip("a CUDA device is visible here")

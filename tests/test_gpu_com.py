@@ -1,4 +1,4 @@
-"""The COM-style drop-in surface (include/whisper_b200_com.h) on a B200: loadModel -> createContext -> fullDefaultParams -> runFull ->
+"""The COM-style drop-in surface (include/whisper_b200_com.h) on an H100: loadModel -> createContext -> fullDefaultParams -> runFull ->
 getResults, exactly the call sequence of the reference's CLI (Examples/main/main.cpp:210-318), driven through the flat wspc_*
 helpers (ctypes cannot call C++ vtables).  The transcription driver is compared with the reference's whisper_full()
 (Whisper/source/whisper.cpp:2765-3125) via fixtures generated from oracle/_ref (tests/golden/full_runs.npz, scripted models)."""

@@ -1,4 +1,4 @@
-"""Kernel-level numerics on a B200, through the C ABI test hooks: the tcgen05 GEMM, the tcgen05 flash attention, the skinny
+"""Kernel-level numerics on an H100, through the C ABI test hooks: the wgmma GEMM, the wgmma flash attention, the skinny
 (decoder) GEMM and LayerNorm, each against a plain numpy reference of the same arithmetic (f16 operands, f32 accumulate)."""
 import numpy as np
 import pytest

@@ -1,6 +1,6 @@
 """The voice activity detector behind iContext::runCapture (whisper_b200/csrc/vad.h, host-only) against the reference's
 (Whisper/Whisper/voiceActivityDetection.cpp): golden vectors generated from the reference's own code (tests/golden/vad.npz,
-tests/golden/make_vad_golden.py), and the live reference library when oracle/_ref/liboracle_vad.so is present.  Integer results
+tests/golden/make_vad_golden.py, and more seeds in tests/golden/reference_extra.npz).  Integer results
 (sample positions): must be identical.  The one stated difference of the pin: the reference build here evaluates its FFT twiddles with
 sinf / cosf in place of DirectXMath's XMScalarSinCos polynomial (oracle/shim/stdafx.h)."""
 import ctypes as C
@@ -13,7 +13,6 @@ from tests.golden.make_vad_golden import N_SIGNALS, drive, vad_signal
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SHIM = os.path.join(HERE, "boundary", "_build", "libvad_test.so")
-REF = os.path.join(os.path.dirname(HERE), "oracle", "_ref", "liboracle_vad.so")
 
 
 def _ours():
@@ -36,12 +35,12 @@ def test_golden_vectors_discriminate():
     assert any(g[k][-1] == 0 for k in g.files) or any(0 in g[k].tolist() for k in g.files)   # ... and "no speech" occurs
 
 
-def test_detector_matches_live_reference():
-    if not os.path.exists(REF):
-        pytest.skip("oracle/_ref/liboracle_vad.so not built (needs /root/reference at build time)")
-    ref, ours = C.CDLL(REF), _ours()
-    for seed in range(100, 130):
-        assert drive(ours, "wvad", seed) == drive(ref, "ora_vad", seed), seed
+def test_detector_matches_reference_more_seeds():
+    from tests.golden.make_reference_extra import VAD_SEEDS
+    g = np.load(os.path.join(HERE, "golden", "reference_extra.npz"))
+    ours = _ours()
+    for seed in VAD_SEEDS:
+        assert drive(ours, "wvad", seed) == g["vad_s%d" % seed].tolist(), seed
 
 
 def test_features_of_known_frames():

@@ -1,6 +1,6 @@
 // Issue rate of the conversion instructions the decoder's f16 V^T*P chains are made of (HADD2.F32 = f16 -> f32, F2FP.F16.F32.PACK_AB =
 // f32 -> f16) against FFMA, per SM: 8 warps x 8 independent streams per thread, so that latency is hidden and only the pipe counts.
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o cvt_rate cvt_rate.cu ; run on the GPU box
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o cvt_rate cvt_rate.cu ; run on an H100
 #include <cstdio>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -47,8 +47,8 @@ template<int MODE>
 void run( const char* name, float* out, long long* cyc )
 {
 	const int iters = 4096;
-	k<MODE><<<148, 256>>>( out, iters, cyc );
-	k<MODE><<<148, 256>>>( out, iters, cyc );
+	k<MODE><<<132, 256>>>( out, iters, cyc );
+	k<MODE><<<132, 256>>>( out, iters, cyc );
 	cudaDeviceSynchronize();
 	long long c;
 	cudaMemcpy( &c, cyc, 8, cudaMemcpyDeviceToHost );
@@ -58,7 +58,7 @@ void run( const char* name, float* out, long long* cyc )
 int main()
 {
 	float* out; long long* cyc;
-	cudaMalloc( &out, 148 * 256 * 4 ); cudaMalloc( &cyc, 8 );
+	cudaMalloc( &out, 132 * 256 * 4 ); cudaMalloc( &cyc, 8 );
 	run<0>( "FFMA", out, cyc );
 	run<2>( "f32->f16->f32 (F2FP + HADD2.F32)", out, cyc );
 	run<3>( "chain step (F2FP + HADD2.F32 + FFMA)", out, cyc );

@@ -21,7 +21,7 @@ METRICS = [
     ("L2 hit %", "lts__t_sector_hit_rate.pct"),
     ("SM % of peak", "sm__throughput.avg.pct_of_peak_sustained_elapsed"),
     ("tensor pipe % (elapsed)", "sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_elapsed"),
-    ("tcgen05 f16->f32 path %", "sm__ops_path_tensor_op_utchmma_src_fp16_dst_fp32_sparsity_off.avg.pct_of_peak_sustained_elapsed"),
+    ("wgmma f16 path %", "sm__ops_path_tensor_op_hgmma_src_fp16_sparsity_off.avg.pct_of_peak_sustained_elapsed"),
     ("mma.sync f16->f32 path %", "sm__ops_path_tensor_op_hmma_src_fp16_dst_fp32_sparsity_off.avg.pct_of_peak_sustained_elapsed"),
     ("achieved occupancy %", "sm__warps_active.avg.pct_of_peak_sustained_active"),
     ("ipc (active)", "smsp__inst_executed.avg.per_cycle_active"),

@@ -1,17 +1,14 @@
-// Fused flash attention for the Whisper encoder on sm_100a (non-causal, head dim 64, T = 1500).
+// Fused flash attention for the Whisper encoder on sm_90a (non-causal, head dim 64, T = 1500).
 //
 // Replaces flashAttention.hlsl / the mulMatTiled -> softMax -> mulMatTiled chain the reference actually runs
 // (Whisper/ML/Context.ops.cpp:194-227) and the CPU oracle's ggml_compute_forward_flash_attn_f16 (Whisper/source/ggml.c:5912-6097):
 //   S = (K q) / sqrt(64)  (f16 x f16 -> f32),  P = softmax(S),  P rounded to f16,  O = V^T P  (f16 x f16 -> f32).
-// Here: one CTA = 128 queries of one (chunk, head); K/V^T tiles of 128 keys arrive by TMA; S = Q K^T and O_tile = P V are
-// tcgen05.mma with accumulators in TMEM; the online softmax runs one query row per thread (no shuffles): the whole 128-wide score row
-// is pulled into registers with four TMEM loads in flight and handled in ONE pass.  The running output stays IN TMEM: P*V of every
-// tile accumulates onto it, relative to a per-row reference maximum that is only moved when a tile's maximum exceeds it by more than
-// 2^8 (then the thread rescales its own TMEM lane: tcgen05.ld / multiply / tcgen05.st — a handful of times per row, in the first
-// tiles).  So a tile no longer waits for its own P*V, reads O back and rescales 64 values: P*V of tile j runs behind the score load
-// and the row maximum of tile j+1, and only the writes of the next P wait for it.  The scores of tile j+1 are issued right behind
-// P*V of tile j; V^T tiles are double-buffered.  Two CTAs co-reside per SM (97 KB smem, 256 TMEM columns each) so one CTA's
-// softmax also overlaps the other's MMAs.
+// Here: one CTA = 128 queries of one (chunk, head), two warpgroups of 64 queries each; K / V^T tiles of 128 keys arrive by TMA,
+// double-buffered, the loads of tile j+2 issued as soon as tile j is consumed.  S = Q K^T is wgmma with A and B in shared memory
+// and the scores in registers; the online softmax runs on the accumulator fragments (a row's 128 scores are spread over the four
+// threads of a quad: two shuffles per reduction), and P is converted in registers straight into the A fragments of O += P V
+// (wgmma with A from registers), so P never goes through shared memory.  O stays in registers and is rescaled when the row maximum
+// grows.  Two CTAs co-reside per SM (81 KB smem each), so one CTA's softmax overlaps the other's MMAs.
 //
 // Rounding points kept from the oracle: Q, K, V and P are f16, all accumulation is f32.  Deliberate difference: exp is
 // exp2f (not the oracle's f16 exp LUT, ggml.c:6065-6067) and P is rounded before the 1/sum normalisation (the oracle rounds after, :6082).
@@ -21,306 +18,181 @@
 
 namespace attn
 {
-	constexpr int TQ = 128;      // queries per CTA
+	constexpr int TQ = 128;      // queries per CTA (two warpgroups of 64)
 	constexpr int TK = 128;      // keys per tile
 	constexpr int HD = 64;       // head dim
 	constexpr int SQ_BYTES = TQ * HD * 2;         // 16 KB
-	constexpr int SK_BYTES = TK * HD * 2;         // 16 KB
-	constexpr int SV_BYTES = HD * TK * 2;         // 16 KB, two [64][64] sub-tiles
-	constexpr int SP_BYTES = TQ * TK * 2;         // 32 KB, two [128][64] sub-tiles
-	constexpr int SMEM_BYTES = SQ_BYTES + SK_BYTES + 2 * SV_BYTES + SP_BYTES + 128 + 1024;
-	constexpr float REF_SLACK = 8.0f;             // a row's reference may lag its running maximum by this much (log2 units): P <= 256
-	constexpr uint32_t TMEM_COLS = 256;           // S: [0,128)  O tile: [128,192)
+	constexpr int SK_BYTES = TK * HD * 2;         // 16 KB per buffer
+	constexpr int SV_BYTES = HD * TK * 2;         // 16 KB per buffer, two [64][64] sub-tiles
+	constexpr int SMEM_BYTES = SQ_BYTES + 2 * SK_BYTES + 2 * SV_BYTES + 128 + 1024;
 
 	// 2^x on the MUFU pipe without exp2f's range-reduction wrapper (x <= 0 here; results below 2^-126 may flush to zero, far below
-	// the f16 P that is kept).  The wrapper cost ~12 extra instructions per score: the kernel was instruction-issue bound (54 %).
+	// the f16 P that is kept).
 	__device__ __forceinline__ float ex2Approx( float x )
 	{
 		float y;
 		asm( "ex2.approx.ftz.f32 %0, %1;" : "=f"( y ) : "f"( x ) );
 		return y;
 	}
-	__device__ __forceinline__ float max3( float a, float b, float c )
+	__device__ __forceinline__ uint32_t packHalf2( float lo, float hi )
 	{
-		float y;
-		asm( "max.f32 %0, %1, %2, %3;" : "=f"( y ) : "f"( a ), "f"( b ), "f"( c ) );
-		return y;
+		__half2 h = __floats2half2_rn( lo, hi );
+		return *reinterpret_cast<uint32_t*>( &h );
+	}
+	__device__ __forceinline__ float quadMax( float v )
+	{
+		v = fmaxf( v, __shfl_xor_sync( 0xffffffffu, v, 1 ) );
+		return fmaxf( v, __shfl_xor_sync( 0xffffffffu, v, 2 ) );
+	}
+	__device__ __forceinline__ float quadSum( float v )
+	{
+		v += __shfl_xor_sync( 0xffffffffu, v, 1 );
+		return v + __shfl_xor_sync( 0xffffffffu, v, 2 );
 	}
 
-	__global__ void __launch_bounds__( 128, 2 )
+	__global__ void __launch_bounds__( 256, 2 )
 		attn_enc_kernel( const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapVt, EncParams p )
 	{
 		extern __shared__ uint8_t smem_raw[];
 		uint8_t* smem = reinterpret_cast<uint8_t*>( ( reinterpret_cast<uintptr_t>( smem_raw ) + 1023 ) & ~(uintptr_t)1023 );
 		uint8_t* sQ = smem;
-		uint8_t* sK = sQ + SQ_BYTES;
-		uint8_t* sV = sK + SK_BYTES;
-		uint8_t* sP = sV + 2 * SV_BYTES;              // (two V^T buffers)
-		uint64_t* bars = reinterpret_cast<uint64_t*>( sP + SP_BYTES );
+		uint8_t* sK = sQ + SQ_BYTES;                  // [2]
+		uint8_t* sV = sK + 2 * SK_BYTES;              // [2]
+		uint64_t* bars = reinterpret_cast<uint64_t*>( sV + 2 * SV_BYTES );
 		uint64_t* bar_q = bars + 0;
-		uint64_t* bar_k = bars + 1;
-		uint64_t* bar_v = bars + 2;                   // [2]: one per V^T buffer
-		uint64_t* bar_s = bars + 4;
-		uint64_t* bar_o = bars + 5;
-		uint32_t* tmem_slot = reinterpret_cast<uint32_t*>( bars + 6 );
+		uint64_t* bar_k = bars + 1;                   // [2]: one per K buffer
+		uint64_t* bar_v = bars + 3;                   // [2]: one per V^T buffer
 
 		const int tid = threadIdx.x;
-		const int warp = tid >> 5;
+		const int lane = tid & 31;
+		const int wg = tid >> 7;                      // warpgroup: queries [64 wg, 64 wg + 64) of the tile
+		const int wq = ( tid >> 5 ) & 3;
 		const int q0 = blockIdx.x * TQ;
 		const int bh = blockIdx.y;
 		const int nkv = ( p.T + TK - 1 ) / TK;
 
+		auto loadKV = [ & ]( int j ) {
+			const int buf = j & 1;
+			ptx::mbar_expect_tx( bar_k + buf, SK_BYTES );
+			ptx::tma_load_2d( sK + buf * SK_BYTES, &mapK, bar_k + buf, 0, bh * p.T + j * TK );
+			ptx::mbar_expect_tx( bar_v + buf, SV_BYTES );
+			ptx::tma_load_2d( sV + buf * SV_BYTES, &mapVt, bar_v + buf, j * TK, bh * HD );
+			ptx::tma_load_2d( sV + buf * SV_BYTES + SV_BYTES / 2, &mapVt, bar_v + buf, j * TK + 64, bh * HD );
+		};
 		if( tid == 0 )
 		{
 			ptx::prefetch_tensormap( &mapQ );
 			ptx::prefetch_tensormap( &mapK );
 			ptx::prefetch_tensormap( &mapVt );
-			for( int i = 0; i < 6; i++ )
+			for( int i = 0; i < 5; i++ )
 				ptx::mbar_init( &bars[ i ], 1 );
 			ptx::fence_barrier_init();
-		}
-		if( warp == 0 )
-		{
-			__syncwarp();
-			ptx::tmem_alloc( tmem_slot, TMEM_COLS );
-			ptx::tmem_relinquish();
-		}
-		ptx::tc_fence_before();
-		__syncthreads();
-		ptx::tc_fence_after();
-		const uint32_t tmem_base = *tmem_slot;
-		const uint32_t tmem_S = tmem_base;
-		const uint32_t tmem_O = tmem_base + 128;
-
-		if( tid == 0 )
-		{
 			ptx::mbar_expect_tx( bar_q, SQ_BYTES );
 			ptx::tma_load_2d( sQ, &mapQ, bar_q, 0, bh * p.T + q0 );
-			ptx::mbar_expect_tx( bar_k, SK_BYTES );
-			ptx::tma_load_2d( sK, &mapK, bar_k, 0, bh * p.T );
-			ptx::mbar_expect_tx( bar_v, SV_BYTES );
-			ptx::tma_load_2d( sV, &mapVt, bar_v, 0, bh * HD );
-			ptx::tma_load_2d( sV + SV_BYTES / 2, &mapVt, bar_v, 64, bh * HD );
-			if( nkv > 1 )
-			{
-				ptx::mbar_expect_tx( bar_v + 1, SV_BYTES );
-				ptx::tma_load_2d( sV + SV_BYTES, &mapVt, bar_v + 1, TK, bh * HD );
-				ptx::tma_load_2d( sV + SV_BYTES + SV_BYTES / 2, &mapVt, bar_v + 1, TK + 64, bh * HD );
-			}
+			loadKV( 0 );
+			if( nkv > 1 ) loadKV( 1 );
 		}
+		__syncthreads();
 
-		constexpr uint32_t idescS = ptx::umma_idesc_f16( TQ, TK );
-		constexpr uint32_t idescO = ptx::umma_idesc_f16( TQ, HD );
-
-		float m_ref = -INFINITY;     // reference maximum of this row's O (in TMEM) and l: P = 2^((s - m_ref) * c)
-		float l_run = 0.0f;
-		const uint32_t lane_base = (uint32_t)( warp * 32 ) << 16;   // this warp's TMEM lane quadrant
-		const int r = tid;                                          // my query row inside the tile
 		const float c = p.scale_log2;
-
-		// first S tile; every later one is issued right behind the previous tile's P*V (see below)
-		if( tid == 0 )
-		{
-			ptx::mbar_wait( bar_q, 0 );
-			ptx::mbar_wait( bar_k, 0 );
-			ptx::tc_fence_after();
-			const uint64_t da = ptx::umma_desc_sw128( ptx::smem_u32( sQ ) );
-			const uint64_t db = ptx::umma_desc_sw128( ptx::smem_u32( sK ) );
+		const int qd = lane & 3;                      // column pair 2qd of every 8-column block
+		float o[ HD / 2 ];                            // O rows (r0, r0 + 8): o[4n + 0/1] row r0, o[4n + 2/3] row r0 + 8, columns 8n + 2qd
 #pragma unroll
-			for( int k = 0; k < HD / 16; k++ )
-				ptx::umma_f16( tmem_S, da + (uint64_t)( k * 2 ), db + (uint64_t)( k * 2 ), idescS, k != 0 ? 1u : 0u );
-			ptx::umma_commit( bar_s );
-		}
-		__syncwarp();
+		for( int i = 0; i < HD / 2; i++ ) o[ i ] = 0.0f;
+		float mRun[ 2 ] = { -INFINITY, -INFINITY };   // running row maxima (raw scores)
+		float lPart[ 2 ] = { 0.0f, 0.0f };            // this thread's share of the row sums, relative to mRun
+		const uint64_t dq = ptx::gmma_desc_sw128( ptx::smem_u32( sQ + wg * 64 * 128 ) );
+		ptx::mbar_wait( bar_q, 0 );
 
 		for( int j = 0; j < nkv; j++ )
 		{
-			const uint32_t ph = (uint32_t)( j & 1 );
-			ptx::mbar_wait( bar_s, ph );
-			ptx::tc_fence_after();
-			if( tid == 0 && j + 1 < nkv )
+			const int buf = j & 1;
+			const uint32_t ph = (uint32_t)( ( j >> 1 ) & 1 );
+			ptx::mbar_wait( bar_k + buf, ph );
+			float s[ TK / 2 ];
 			{
-				// K tile consumed: fetch the next one behind this tile's softmax
-				ptx::mbar_expect_tx( bar_k, SK_BYTES );
-				ptx::tma_load_2d( sK, &mapK, bar_k, 0, bh * p.T + ( j + 1 ) * TK );
-			}
-			__syncwarp();
-
-			const int kv_base = j * TK;
-			const int nvalid = p.T - kv_base;   // columns >= nvalid are padding / the next head's rows
-			const bool fullTile = nvalid >= TK; // only the last tile of a head has padding columns
-
-			// the whole score row of this thread's query in registers: four TMEM loads in flight, ONE wait, one pass
-			// (round 1 read the row twice, 32 columns at a time with a wait each: TMEM latency x 8 on the critical path of every tile)
-			uint32_t sc[ TK ];
+				const uint64_t dk = ptx::gmma_desc_sw128( ptx::smem_u32( sK + buf * SK_BYTES ) );
+				ptx::wgmma_fence();
 #pragma unroll
-			for( int ch = 0; ch < TK / 32; ch++ ) ptx::tmem_ld_32x32( tmem_S + lane_base + (uint32_t)( ch * 32 ), sc + ch * 32 );
-			ptx::tmem_ld_wait();
-			float mx = -INFINITY;
-			if( fullTile )
-			{
-#pragma unroll
-				for( int i = 0; i < TK; i += 2 ) mx = max3( mx, __uint_as_float( sc[ i ] ), __uint_as_float( sc[ i + 1 ] ) );
-			}
-			else
-			{
-#pragma unroll
-				for( int i = 0; i < TK; i++ )
-					if( i < nvalid ) mx = fmaxf( mx, __uint_as_float( sc[ i ] ) );
+				for( int k = 0; k < HD / 16; k++ )
+					ptx::wgmma_m64n128k16_ss( s, dq + (uint64_t)( k * 2 ), dk + (uint64_t)( k * 2 ), k != 0 ? 1u : 0u );
+				ptx::wgmma_commit();
+				ptx::wgmma_wait<0>();
+				ptx::fence_regs<TK / 2>( s );
 			}
 
-			// P*V of the previous tile has to be done before its P is overwritten (and before O is touched); it ran behind the loads and
-			// the row maximum above
-			if( j > 0 )
+			// columns >= nvalid are padding / the next head's rows (only in the last tile of a head)
+			const int nvalid = p.T - j * TK;
+			if( nvalid < TK )
 			{
-				ptx::mbar_wait( bar_o, ph ^ 1u );
-				ptx::tc_fence_after();
-				if( tid == 0 && j + 1 < nkv )
+#pragma unroll
+				for( int i = 0; i < TK / 2; i++ )
+					if( 8 * ( i >> 2 ) + 2 * qd + ( i & 1 ) >= nvalid ) s[ i ] = -INFINITY;
+			}
+			float mx[ 2 ] = { -INFINITY, -INFINITY };
+#pragma unroll
+			for( int i = 0; i < TK / 2; i++ ) mx[ ( i >> 1 ) & 1 ] = fmaxf( mx[ ( i >> 1 ) & 1 ], s[ i ] );
+			float f[ 2 ], nmc[ 2 ];
+#pragma unroll
+			for( int r = 0; r < 2; r++ )
+			{
+				const float mNew = fmaxf( mRun[ r ], quadMax( mx[ r ] ) );
+				f[ r ] = ex2Approx( ( mRun[ r ] - mNew ) * c );
+				mRun[ r ] = mNew;
+				nmc[ r ] = -mNew * c;
+				lPart[ r ] *= f[ r ];
+			}
+#pragma unroll
+			for( int i = 0; i < HD / 2; i++ ) o[ i ] *= f[ ( i >> 1 ) & 1 ];
+
+			// probabilities -> f16 A fragments: k-slice kk (keys 16kk..16kk+15) is score blocks 2kk and 2kk+1
+			uint32_t pa[ TK / 4 ];
+#pragma unroll
+			for( int i = 0; i < TK / 2; i += 2 )
+			{
+				const int r = ( i >> 1 ) & 1;
+				const float e0 = ex2Approx( fmaf( s[ i ], c, nmc[ r ] ) );
+				const float e1 = ex2Approx( fmaf( s[ i + 1 ], c, nmc[ r ] ) );
+				lPart[ r ] += e0 + e1;
+				pa[ i >> 1 ] = packHalf2( e0, e1 );
+			}
+
+			ptx::mbar_wait( bar_v + buf, ph );
+			{
+				const uint32_t sv = ptx::smem_u32( sV + buf * SV_BYTES );
+				ptx::fence_regs<HD / 2>( o );
+				ptx::wgmma_fence();
+#pragma unroll
+				for( int kk = 0; kk < TK / 16; kk++ )
 				{
-					// the V^T buffer of tile j-1 is free: fetch tile j+1 into it
-					uint64_t* bv = bar_v + ( ( j + 1 ) & 1 );
-					uint8_t* dv = sV + ( ( j + 1 ) & 1 ) * SV_BYTES;
-					ptx::mbar_expect_tx( bv, SV_BYTES );
-					ptx::tma_load_2d( dv, &mapVt, bv, ( j + 1 ) * TK, bh * HD );
-					ptx::tma_load_2d( dv + SV_BYTES / 2, &mapVt, bv, ( j + 1 ) * TK + 64, bh * HD );
+					const uint64_t dv = ptx::gmma_desc_sw128( sv + (uint32_t)( ( kk >> 2 ) * ( SV_BYTES / 2 ) ) ) + (uint64_t)( ( kk & 3 ) * 2 );
+					ptx::wgmma_m64n64k16_rs( o, pa + kk * 4, dv, 1u );
 				}
-				__syncwarp();
-				// move the reference of a row whose maximum ran away from it: O (this thread's TMEM lane) and l shrink by 2^(old - new).
-				// Warp-uniform (the TMEM accesses are collective); rows that stay get the factor 1.
-				const bool move = ( mx - m_ref ) * c > REF_SLACK;
-				if( __any_sync( 0xffffffffu, move ) )
-				{
-					const float f = move ? ex2Approx( ( m_ref - mx ) * c ) : 1.0f;
-#pragma unroll
-					for( int hh = 0; hh < HD / 32; hh++ )
-					{
-						uint32_t rg[ 32 ];
-						ptx::tmem_ld_32x32( tmem_O + lane_base + (uint32_t)( hh * 32 ), rg );
-						ptx::tmem_ld_wait();
-#pragma unroll
-						for( int i = 0; i < 32; i++ ) rg[ i ] = __float_as_uint( __uint_as_float( rg[ i ] ) * f );
-						ptx::tmem_st_32x32( tmem_O + lane_base + (uint32_t)( hh * 32 ), rg );
-					}
-					ptx::tmem_st_wait();
-					l_run *= f;
-					if( move ) m_ref = mx;
-				}
+				ptx::wgmma_commit();
+				ptx::wgmma_wait<0>();
+				ptx::fence_regs<HD / 2>( o );
 			}
-			else
-				m_ref = mx;
-			const float nmc = -m_ref * c;
 
-			// probabilities -> f16 -> swizzled smem (A operand of P*V)
-			float lsum = 0.0f;
-#pragma unroll
-			for( int ch = 0; ch < TK / 32; ch++ )
-			{
-				uint8_t* sub = sP + ( ch >> 1 ) * ( SP_BYTES / 2 ) + r * 128;
-#pragma unroll
-				for( int g = 0; g < 4; g++ )
-				{
-					float e[ 8 ];
-#pragma unroll
-					for( int i = 0; i < 8; i++ )
-					{
-						const int col = ch * 32 + g * 8 + i;
-						const float v = ex2Approx( fmaf( __uint_as_float( sc[ col ] ), c, nmc ) );
-						e[ i ] = ( fullTile || col < nvalid ) ? v : 0.0f;
-						lsum += e[ i ];
-					}
-					const int chunk16 = ( ( ch & 1 ) * 4 + g ) ^ ( r & 7 );
-					__half2 h0 = __floats2half2_rn( e[ 0 ], e[ 1 ] );
-					__half2 h1 = __floats2half2_rn( e[ 2 ], e[ 3 ] );
-					__half2 h2 = __floats2half2_rn( e[ 4 ], e[ 5 ] );
-					__half2 h3 = __floats2half2_rn( e[ 6 ], e[ 7 ] );
-					uint4 u;
-					u.x = *reinterpret_cast<uint32_t*>( &h0 );
-					u.y = *reinterpret_cast<uint32_t*>( &h1 );
-					u.z = *reinterpret_cast<uint32_t*>( &h2 );
-					u.w = *reinterpret_cast<uint32_t*>( &h3 );
-					*reinterpret_cast<uint4*>( sub + chunk16 * 16 ) = u;
-				}
-			}
-			l_run += lsum;
-
-			ptx::fence_proxy_async();   // generic-proxy smem writes -> visible to the tensor core (async proxy)
-			ptx::tc_fence_before();
-			__syncthreads();            // P complete, every thread has its S row in registers (the S columns are free again), O lanes settled
-
-			if( tid == 0 )
-			{
-				ptx::tc_fence_after();
-				ptx::mbar_wait( bar_v + ( j & 1 ), (uint32_t)( ( j >> 1 ) & 1 ) );
-				ptx::tc_fence_after();
-				const uint8_t* sVj = sV + ( j & 1 ) * SV_BYTES;
-#pragma unroll
-				for( int k = 0; k < TK / 16; k++ )
-				{
-					const uint64_t da = ptx::umma_desc_sw128( ptx::smem_u32( sP + ( k >> 2 ) * ( SP_BYTES / 2 ) ) ) + (uint64_t)( ( k & 3 ) * 2 );
-					const uint64_t db = ptx::umma_desc_sw128( ptx::smem_u32( sVj + ( k >> 2 ) * ( SV_BYTES / 2 ) ) ) + (uint64_t)( ( k & 3 ) * 2 );
-					ptx::umma_f16( tmem_O, da, db, idescO, ( k != 0 || j != 0 ) ? 1u : 0u );   // O accumulates over the tiles
-				}
-				ptx::umma_commit( bar_o );
-				if( j + 1 < nkv )
-				{
-					// the NEXT tile's scores right behind this P*V
-					ptx::mbar_wait( bar_k, ph ^ 1u );
-					ptx::tc_fence_after();
-					const uint64_t dq = ptx::umma_desc_sw128( ptx::smem_u32( sQ ) );
-					const uint64_t dk = ptx::umma_desc_sw128( ptx::smem_u32( sK ) );
-#pragma unroll
-					for( int k = 0; k < HD / 16; k++ )
-						ptx::umma_f16( tmem_S, dq + (uint64_t)( k * 2 ), dk + (uint64_t)( k * 2 ), idescS, k != 0 ? 1u : 0u );
-					ptx::umma_commit( bar_s );
-				}
-			}
-			__syncwarp();
+			// both warpgroups are done with buffer `buf`: refill it with tile j+2
+			__syncthreads();
+			if( tid == 0 && j + 2 < nkv ) loadKV( j + 2 );
 		}
 
-		// the last P*V, then O / l as f16
-		ptx::mbar_wait( bar_o, (uint32_t)( ( nkv - 1 ) & 1 ) );
-		ptx::tc_fence_after();
-		float o_acc[ HD ];
-		{
-			uint32_t rg[ HD ];
-			ptx::tmem_ld_32x32( tmem_O + lane_base, rg );
-			ptx::tmem_ld_32x32( tmem_O + lane_base + 32u, rg + 32 );
-			ptx::tmem_ld_wait();
+		// O / l as f16, merged-heads layout [chunk][t][h*64 + e]
+		const int b = bh / p.H;
+		const int h = bh - b * p.H;
 #pragma unroll
-			for( int i = 0; i < HD; i++ ) o_acc[ i ] = __uint_as_float( rg[ i ] );
-		}
-		ptx::tc_fence_before();
-
-		// write O / l as f16, merged-heads layout [chunk][t][h*64 + e]
-		const int t = q0 + r;
-		if( t < p.T )
+		for( int r = 0; r < 2; r++ )
 		{
-			const int b = bh / p.H;
-			const int h = bh - b * p.H;
-			const float inv = 1.0f / l_run;
-			__half* dst = p.out + ( (size_t)b * p.T + t ) * p.d + h * HD;
-#pragma unroll
-			for( int g = 0; g < 8; g++ )
+			const int t = q0 + wg * 64 + wq * 16 + ( lane >> 2 ) + 8 * r;
+			const float inv = 1.0f / quadSum( lPart[ r ] );
+			if( t < p.T )
 			{
-				__half2 h0 = __floats2half2_rn( o_acc[ g * 8 + 0 ] * inv, o_acc[ g * 8 + 1 ] * inv );
-				__half2 h1 = __floats2half2_rn( o_acc[ g * 8 + 2 ] * inv, o_acc[ g * 8 + 3 ] * inv );
-				__half2 h2 = __floats2half2_rn( o_acc[ g * 8 + 4 ] * inv, o_acc[ g * 8 + 5 ] * inv );
-				__half2 h3 = __floats2half2_rn( o_acc[ g * 8 + 6 ] * inv, o_acc[ g * 8 + 7 ] * inv );
-				uint4 u;
-				u.x = *reinterpret_cast<uint32_t*>( &h0 );
-				u.y = *reinterpret_cast<uint32_t*>( &h1 );
-				u.z = *reinterpret_cast<uint32_t*>( &h2 );
-				u.w = *reinterpret_cast<uint32_t*>( &h3 );
-				reinterpret_cast<uint4*>( dst )[ g ] = u;
+				__half* dst = p.out + ( (size_t)b * p.T + t ) * p.d + h * HD + 2 * qd;
+#pragma unroll
+				for( int n = 0; n < HD / 8; n++ )
+					*reinterpret_cast<uint32_t*>( dst + 8 * n ) = packHalf2( o[ 4 * n + 2 * r ] * inv, o[ 4 * n + 2 * r + 1 ] * inv );
 			}
-		}
-
-		ptx::tc_fence_before();
-		__syncthreads();
-		if( warp == 0 )
-		{
-			ptx::tc_fence_after();
-			ptx::tmem_dealloc( tmem_base, TMEM_COLS );
 		}
 	}
 
@@ -332,7 +204,7 @@ namespace attn
 			if( e != cudaSuccess ) return e;
 		}
 		dim3 grid( ( p.T + TQ - 1 ) / TQ, p.nBH );
-		attn_enc_kernel<<<grid, 128, SMEM_BYTES, stream>>>( mapQ, mapK, mapVt, p );
+		attn_enc_kernel<<<grid, 256, SMEM_BYTES, stream>>>( mapQ, mapK, mapVt, p );
 		return cudaGetLastError();
 	}
 }

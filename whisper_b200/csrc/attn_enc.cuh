@@ -1,4 +1,4 @@
-// Encoder flash attention (tcgen05) — see attn_enc.cu.
+// Encoder flash attention (wgmma) — see attn_enc.cu.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>

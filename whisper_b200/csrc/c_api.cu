@@ -36,7 +36,7 @@ namespace
 
 extern "C" {
 
-const char* wsp_version( void ) { return "whisper_b200 0.1 (sm_100a: tcgen05 + TMA)"; }
+const char* wsp_version( void ) { return "whisper_b200 0.1 (sm_90a: wgmma + TMA)"; }
 const char* wsp_last_error( void ) { return g_lastError.c_str(); }
 int32_t wsp_device_count( void )
 {
@@ -428,7 +428,7 @@ void wsp_host_free( void* p ) { if( p ) cudaFreeHost( p ); }
 // ===================================================================================================================
 // kernel-level test hooks
 // ===================================================================================================================
-static wsp_status requireSm100( int device )
+static wsp_status requireSm90( int device )
 {
 	int count = 0;
 	WSP_CUDA( cudaGetDeviceCount( &count ) );
@@ -436,7 +436,7 @@ static wsp_status requireSm100( int device )
 	WSP_CUDA( cudaSetDevice( device ) );
 	cudaDeviceProp prop;
 	WSP_CUDA( cudaGetDeviceProperties( &prop, device ) );
-	if( prop.major != 10 ) return fail( WSP_E_CUDA, "needs an sm_100a device" );
+	if( prop.major != 9 || prop.minor != 0 ) return fail( WSP_E_CUDA, "needs an sm_90a device" );
 	return WSP_OK;
 }
 
@@ -444,7 +444,7 @@ wsp_status wsp_test_gemm( int32_t device, int32_t M, int32_t N, int32_t K, const
 {
 	if( !A || !B || !D ) return fail( WSP_E_POINTER, "A/B/D" );
 	if( M < 1 || N < 1 || K < 8 || ( K % 8 ) != 0 || ( bn != 128 && bn != 256 ) ) return fail( WSP_E_INVALIDARG, "shape (K must be a multiple of 8)" );
-	WSP_CHECK( requireSm100( device ) );
+	WSP_CHECK( requireSm90( device ) );
 	cudaDeviceProp prop;
 	WSP_CUDA( cudaGetDeviceProperties( &prop, device ) );
 	DevTmp<__half> dA, dB;
@@ -494,7 +494,7 @@ wsp_status wsp_test_attention( int32_t device, int32_t BH, int32_t T, const uint
 {
 	if( !Q || !K || !V || !out ) return fail( WSP_E_POINTER, "Q/K/V/out" );
 	if( BH < 1 || T < 1 ) return fail( WSP_E_INVALIDARG, "shape" );
-	WSP_CHECK( requireSm100( device ) );
+	WSP_CHECK( requireSm90( device ) );
 	const int Tp = ( ( T + 127 ) / 128 ) * 128;
 	const size_t n = (size_t)BH * T * 64;
 	DevTmp<__half> dQ, dK, dV, dVt, dO;
@@ -539,7 +539,7 @@ wsp_status wsp_test_skinny( int32_t device, int32_t nOut, int32_t K, int32_t col
 {
 	if( !W || !X || !out ) return fail( WSP_E_POINTER, "W/X/out" );
 	if( nOut < 1 || K < 32 || K % 32 != 0 || cols < 1 ) return fail( WSP_E_INVALIDARG, "shape (K multiple of 32)" );
-	WSP_CHECK( requireSm100( device ) );
+	WSP_CHECK( requireSm90( device ) );
 	DevTmp<__half> dW, dX;
 	DevTmp<float> dO;
 	WSP_CUDA( dW.alloc( (size_t)nOut * K ) );
@@ -572,7 +572,7 @@ wsp_status wsp_test_skinny( int32_t device, int32_t nOut, int32_t K, int32_t col
 wsp_status wsp_test_layernorm( int32_t device, int32_t rows, int32_t d, const float* x, const float* gamma, const float* beta, uint16_t* out )
 {
 	if( !x || !gamma || !beta || !out ) return fail( WSP_E_POINTER, "x/gamma/beta/out" );
-	WSP_CHECK( requireSm100( device ) );
+	WSP_CHECK( requireSm90( device ) );
 	DevTmp<float> dx, dg, db;
 	DevTmp<__half> dout;
 	WSP_CUDA( dx.alloc( (size_t)rows * d ) ); WSP_CUDA( dg.alloc( d ) ); WSP_CUDA( db.alloc( d ) ); WSP_CUDA( dout.alloc( (size_t)rows * d ) );
@@ -592,7 +592,7 @@ wsp_status wsp_test_sample( int32_t device, int32_t rows, int32_t n_vocab, const
 {
 	if( !logits || !special4 || !out ) return fail( WSP_E_POINTER, "logits/special/out" );
 	if( rows < 1 || rows > 4096 || n_vocab < 8 ) return fail( WSP_E_INVALIDARG, "rows / n_vocab" );
-	WSP_CHECK( requireSm100( device ) );
+	WSP_CHECK( requireSm90( device ) );
 	static_assert( sizeof( wsp_token_data ) == sizeof( kern::TokenData ), "token data layout" );
 	DevTmp<float> dl, dp;
 	DevTmp<int> dflags, dscratch;

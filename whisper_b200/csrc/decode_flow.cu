@@ -34,7 +34,7 @@ namespace kern
 		constexpr int FL_NSMAX = 32;
 		constexpr int FL_MAXT = 1536;
 		constexpr int FL_MAXPARTS = 16;                // reference thread counts whose V^T*P split the kernel reproduces
-		constexpr int FL_SMEM_MAX = 232448;            // 227 KB opt-in limit per CTA on sm_100
+		constexpr int FL_SMEM_MAX = 232448;            // 227 KB opt-in limit per CTA on sm_90
 		constexpr uint32_t SENT32 = 0xFFFFFFFFu;
 
 		template<int D>
@@ -155,7 +155,7 @@ namespace kern
 
 
 		// The reference's f16-accumulated V^T*P (ggml.c:4680-4722, 871-893): y = f16( fma( V[j][e], P[j], y ) ) key by key — three dependent
-		// ALU instructions per key (FFMA -> F2FP.F16.F32 -> HADD2.F32), ~30 cycles, inherent to the reference's arithmetic (staging the
+		// ALU instructions per key (FFMA -> F2FP.F16.F32 -> HADD2.F32), inherent to the reference's arithmetic (staging the
 		// operands of eight keys ahead of the chain changed nothing: it is not load-bound).
 		__device__ __forceinline__ float chainStep( float y, float x, float p ) { return __half2float( __float2half_rn( __fmaf_rn( x, p, y ) ) ); }
 		__device__ __forceinline__ float chainRows( float y, const float* __restrict__ sp, const __half* __restrict__ v, int n )
@@ -237,14 +237,13 @@ namespace kern
 
 		// Scores of n K rows (128 bytes each, contiguous in shared memory) against the query: q . K[r] on the tensor cores, m16n8k16 tiles
 		// of 16 rows, f16 products accumulated in f32 like the reference's ggml_vec_dot_f16 (in another order).  (The first versions did
-		// this on the FMA pipe — 8 lanes per row, then 2 lanes per row with four accumulators: 130 instructions per lane and slot,
-		// 0.41-0.47 us per 128-row slot, 5.6 of the 17.5 us of a cross-attention phase.)  qB = the query pieces of this lane (scorePiece).
+		// this on the FMA pipe — 8 lanes per row, then 2 lanes per row with four accumulators: 130 instructions per lane and slot.)  qB = the query pieces of this lane (scorePiece).
 		// The calling warp takes the tiles tile0, tile0 + tileStep, ..., TI of them at a time: their loads are issued together and their
 		// four-HMMA chains interleaved.  <1>( warp, 8 ) spreads one slot over the eight warps (self-attention: one short slot);
 		// <4>( 0, 1 ) gives a whole 128-row slot to one warp — the way a long run of slots is scored: whatever a warp computes on a slot,
-		// the slot costs it a fixed ~300 cycles of dependent latency (barrier wait -> LDS -> chained HMMAs -> STS -> release), so eight
+		// the slot costs it a fixed stretch of dependent latency (barrier wait -> LDS -> chained HMMAs -> STS -> release), so eight
 		// warps on eight DIFFERENT slots score a resident key memory about twice as fast as eight warps sharing every slot
-		// (cross-attention, 12 slots: 4.6 -> 2.5 us).  Returns the running maximum.
+		// Returns the running maximum.
 		template<int TI>
 		__device__ __forceinline__ float scoreRows( const uint8_t* kc, int n, int jBase, const uint4 ( &qB )[ 2 ], float* sp, int tile0, int tileStep, int lane, float lmax )
 		{
@@ -320,10 +319,10 @@ namespace kern
 			constexpr int N4 = Cfg<D>::N4;
 			const uint4* src = reinterpret_cast<const uint4*>( row );
 			SpinGuard guard;
-			// Probe before reading: four words at the quarter points of the row, polled with back-off, until they are written.  148
+			// Probe before reading: four words at the quarter points of the row, polled with back-off, until they are written.  132
 			// CTAs re-reading whole 32 KB activation blocks while they wait would by themselves saturate the L2 (one round = 4.7 MB,
-			// ~10 TB/s when spinning) and starve the weight stream; the probes cost four sectors per round.  (Measured alternative:
-			// an optimistic full read first, probes only after a miss — every phase 0.3-0.9 us slower: CTAs arrive early as a rule.)
+			// ~10 TB/s when spinning) and starve the weight stream; the probes cost four sectors per round.  (An optimistic
+			// full read first, probes only after a miss, is slower: CTAs arrive early as a rule.)
 			{
 				const uint32_t* w = reinterpret_cast<const uint32_t*>( row ) + ( lane & 3 ) * ( D / 4 ) + D / 8;
 				unsigned ns = 32;
@@ -765,8 +764,7 @@ namespace kern
 
 			// The step is ONE loop over (layer, phase) with a single copy of the weight-streaming GEMV code and a single copy of the
 			// attention code; a switch only fills in their operands.  (The first version of this kernel instantiated the GEMV seven
-			// times: 16 K SASS instructions = 256 KB, every phase started with a cold instruction cache — 1.2-1.5 us for the four
-			// MMA steps of an 8-row unit.  Round 1 measured the same effect on its barrier kernel: 12.4 K -> 7.0 K instructions.)
+			// times: 16 K SASS instructions = 256 KB, every phase started with a cold instruction cache.)
 			enum { PH_QKV = 0, PH_SELF = 1, PH_O = 2, PH_CQ = 3, PH_CROSS = 4, PH_CO = 5, PH_FC1 = 6, PH_FC2 = 7, PH_COUNT = 8 };
 #pragma unroll 1
 			for( int il = 0; il <= L; il++ )
@@ -1023,8 +1021,8 @@ namespace kern
 							{
 								if( u < nb )
 								{
-									// (all units of a pass side by side — wait for their slots together, interleave their HMMA chains — was measured
-									// slower: 96.6 -> 104.7 ms per 100 tokens; the weights of fc1 / fc2 arrive while the first units compute)
+									// (all units of a pass side by side — wait for their slots together, interleave their HMMA chains — is
+									// slower: the weights of fc1 / fc2 arrive while the first units compute)
 									const uint8_t* w = waitSlot( 0 );
 									if( u == 0 && kc == 0 && u0 == 0 ) sub( 2 );
 									const uint8_t* wb = w + (size_t)gq * RS + tq * 16;

@@ -2,9 +2,9 @@
 // logits) for up to 16 chunks, with grid-wide barriers between the data-dependent phases instead of ~190 kernel launches.
 //
 // Why: at batch 8 the step is a chain of ~190 tiny weight-streaming ops (SURVEY.md §7 "Decode latency").  Launched as separate
-// kernels each one costs 5-12 us of launch / drain / first-byte latency while it moves only 2-8 MB, i.e. < 10 % of HBM rate.
+// kernels each one pays launch / drain / first-byte latency while it moves only 2-8 MB, far below the HBM rate.
 // Here one CTA per SM stays resident; every phase is split into small units (8 weight rows, or one (chunk, head)) distributed
-// round-robin over the 148 CTAs; each CTA issues the HBM loads of its NEXT phase (weights / cross-KV, which do not depend on the
+// round-robin over the resident CTAs; each CTA issues the HBM loads of its NEXT phase (weights / cross-KV, which do not depend on the
 // previous phase) BEFORE it waits at the grid barrier, so memory latency overlaps the barrier and the predecessor's tail.
 //
 // Arithmetic is identical to the kernel-per-op path (kernels_decode.cu): f16 x f16 -> f32 through mma.sync.m16n8k16 with the
@@ -96,11 +96,11 @@ namespace kern
 			unsigned* counter;   // [0] arrivals, [32] epoch flag (separate line); zeroed by the launcher
 			unsigned target;
 			unsigned epoch;
-			// (measured alternative: per-CTA epoch slots polled by warp 0 of every CTA, no atomics — arrive got cheaper, 0.5-1.2 us
-			// instead of 0.8-2.1, but observing 148 slots cost more than it saved: decode 167 vs 160 ms)
+			// (alternative: per-CTA epoch slots polled by warp 0 of every CTA, no atomics — arrive gets cheaper, but observing one slot
+			// per SM costs more than it saves)
 			// Split barrier: arrive() right after a phase's last global store, wait() after the next phase's prefetches have been
 			// issued.  (A release-atomic drains the issuing warp's outstanding loads first, so arriving AFTER the prefetch issue put
-			// an HBM round trip on every barrier's critical path: 2.3 -> 0.85 us per barrier, 1862 -> 1638 us per step.)
+			// an HBM round trip on every barrier's critical path.)
 			__device__ __forceinline__ void arrive( unsigned long long* tm = nullptr )
 			{
 				target += gridDim.x;
@@ -206,7 +206,7 @@ namespace kern
 
 		// LayerNorm gamma/beta and the bias entries of this CTA's units of the NEXT phase -> shared memory, requested before the
 		// barrier: per-layer parameters are cold in L2 (every step streams ~2 GB through it), and a DRAM miss on them would sit in the
-		// middle of the post-barrier critical path (measured: 4.5 us per LayerNorm phase without this)
+		// middle of the post-barrier critical path
 		__device__ __forceinline__ void prefetchParams( const GemvOp& op, int K, const Smem& sm, int tid )
 		{
 			if( op.gamma )
@@ -751,7 +751,7 @@ namespace kern
 				return o;
 			};
 			// everything a phase needs that does not depend on the previous phase is requested before the barrier wait
-			// (measured alternative: prefetching these rows into L2 only and loading the registers after the barrier is exactly as fast)
+			// (alternative: prefetching these rows into L2 only and loading the registers after the barrier is exactly as fast)
 			auto prepD = [ & ]( const GemvOp& o ) {
 				loadBatch<D>( wb, o, 0, myUnits<D>( o ), 0, warp, lane );
 				prefetchParams( o, D, sm, tid );

@@ -153,8 +153,8 @@ namespace wsp
 		WSP_CUDA( cudaSetDevice( device ) );
 		cudaDeviceProp prop;
 		WSP_CUDA( cudaGetDeviceProperties( &prop, device ) );
-		if( prop.major != 10 )
-			return fail( WSP_E_CUDA, std::string( "whisper_b200 needs an sm_100a device (tcgen05/TMA); found " ) + prop.name + " sm_" + std::to_string( prop.major ) + std::to_string( prop.minor ) );
+		if( prop.major != 9 || prop.minor != 0 )
+			return fail( WSP_E_CUDA, std::string( "whisper_b200 needs an sm_90a device (wgmma/TMA); found " ) + prop.name + " sm_" + std::to_string( prop.major ) + std::to_string( prop.minor ) );
 
 		std::unique_ptr<Engine> e( new Engine() );
 		e->device = device;

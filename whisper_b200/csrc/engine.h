@@ -1,4 +1,4 @@
-// Engine (weights on one B200) and Context (per-stream state for up to maxBatch independent 30 s chunks).
+// Engine (weights on one H100) and Context (per-stream state for up to maxBatch independent 30 s chunks).
 //
 // Reference counterparts: ModelBuffers (Whisper/Whisper/ModelBuffers.h:8-111) / WhisperModel (loader), and WhisperContext
 // (Whisper/Whisper/WhisperContext.cpp:138-639 — the network definition) with its KeyValueBuffers (KeyValueBuffers.h:7-53).
@@ -62,7 +62,7 @@ namespace wsp
 	struct Engine
 	{
 		int device = 0;
-		int numSMs = 148;
+		int numSMs = 132;
 		HParams hp{};
 		int tokEot = 0, tokSot = 0, tokPrev = 0, tokSolm = 0, tokNot = 0, tokBeg = 0;
 		uint8_t* arena = nullptr;

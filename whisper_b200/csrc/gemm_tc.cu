@@ -1,4 +1,4 @@
-// tcgen05 + TMA GEMM for sm_100a — see gemm_tc.cuh for the design notes.
+// wgmma + TMA GEMM for sm_90a — see gemm_tc.cuh for the design notes.
 #include "gemm_tc.cuh"
 #include "per_device.h"
 #include <stdio.h>
@@ -166,22 +166,15 @@ namespace gemm
 	}
 
 	// ---------------------------------------------------------------------------------------------------------------
-	// Coalesced epilogues.  tcgen05.ld hands every thread one ROW of the accumulator tile, so a direct store makes each warp
-	// instruction touch 32 different rows (16 bytes each): half of every 32-byte sector is wasted and a 128-byte line needs 8
-	// separate instructions (measured: the out-projection GEMM ran at 17 % tensor-pipe utilisation, epilogue-bound).  The
-	// accumulator chunk (32 rows x 32 columns) is therefore transposed through a padded per-warp shared-memory tile so that a
-	// thread owns one COLUMN: every load / store instruction of the warp then covers 32 consecutive elements of one output row.
-	__device__ __forceinline__ void loadResid( const EpiParams& ep, int mBase, int n, float* rs )
-	{
-#pragma unroll
-		for( int rr = 0; rr < 32; rr++ )
-		{
-			const int m = mBase + rr;
-			rs[ rr ] = ( m < ep.M && n < ep.N ) ? ep.resid[ (size_t)m * ep.ld + n ] : 0.0f;
-		}
-	}
+	constexpr int STG_LD = 72;   // staging row stride (floats): the float2 fragment stores of a half-warp hit 32 distinct banks
+
+	// Coalesced epilogues.  Giving every thread one ROW of the tile makes each warp instruction touch 32 different rows (16 bytes
+	// each): half of every 32-byte sector is wasted and a 128-byte line needs 8 separate instructions.  For f32 outputs the
+	// 32 x 32 chunk is therefore read from the staging tile so that a thread owns one COLUMN: every load / store instruction of the
+	// warp then covers 32 consecutive elements of one output row.  `w` points at the thread's column in the staging tile
+	// (row stride STG_LD).
 	template<int MODE>
-	__device__ __forceinline__ void epilogueT( const EpiParams& ep, int mBase, int n, const float* w, const float* rs = nullptr )
+	__device__ __forceinline__ void epilogueT( const EpiParams& ep, int mBase, int n, const float* w )
 	{
 		if( n >= ep.N ) return;
 		if constexpr( MODE == EPI_F32 )
@@ -191,7 +184,7 @@ namespace gemm
 			for( int rr = 0; rr < 32; rr++ )
 			{
 				const int m = mBase + rr;
-				if( m < ep.M ) ep.out_f32[ (size_t)m * ep.ld + n ] = w[ rr ] + b;
+				if( m < ep.M ) ep.out_f32[ (size_t)m * ep.ld + n ] = w[ rr * STG_LD ] + b;
 			}
 		}
 		else if constexpr( MODE == EPI_CONV1 )
@@ -203,7 +196,7 @@ namespace gemm
 			for( int rr = 0; rr < 32; rr++ )
 			{
 				if( cb < ep.nchunks && t < ep.valid_per_chunk )
-					ep.out_a[ (size_t)( mBase + rr + 1 ) * ep.ld + n ] = __float2half_rn( ptx::gelu_f16_semantics( w[ rr ] + b ) );
+					ep.out_a[ (size_t)( mBase + rr + 1 ) * ep.ld + n ] = __float2half_rn( ptx::gelu_f16_semantics( w[ rr * STG_LD ] + b ) );
 				if( ++t == ep.rows_per_chunk ) { t = 0; cb++; }
 			}
 		}
@@ -212,24 +205,29 @@ namespace gemm
 			const float b = ep.bias[ n ];
 			const int cb0 = mBase / ep.rows_per_chunk;
 			const int j0 = mBase - cb0 * ep.rows_per_chunk;
-			// positional rows first (loads must not be serialised behind the stores: pos and out_f32 are both float*)
-			float pe[ 32 ];
-			{
-				int j = j0;
+			// positional rows first, 16 at a time (loads must not be serialised behind the stores: pos and out_f32 are both float*)
 #pragma unroll
-				for( int rr = 0; rr < 32; rr++ )
+			for( int h = 0; h < 32; h += 16 )
+			{
+				float pe[ 16 ];
+				int j = j0 + h, cb = cb0;
+				while( j >= ep.rows_per_chunk ) { j -= ep.rows_per_chunk; cb++; }
 				{
-					pe[ rr ] = j < ep.valid_per_chunk ? ep.pos[ (size_t)j * ep.d + n ] : 0.0f;
-					if( ++j == ep.rows_per_chunk ) j = 0;
-				}
-			}
-			int cb = cb0, j = j0;
+					int jj = j;
 #pragma unroll
-			for( int rr = 0; rr < 32; rr++ )
-			{
-				if( cb < ep.nchunks && j < ep.valid_per_chunk )
-					ep.out_f32[ ( (size_t)cb * ep.T + j ) * ep.ld + n ] = ptx::gelu_f16_semantics( w[ rr ] + b ) + pe[ rr ];
-				if( ++j == ep.rows_per_chunk ) { j = 0; cb++; }
+					for( int rr = 0; rr < 16; rr++ )
+					{
+						pe[ rr ] = jj < ep.valid_per_chunk ? ep.pos[ (size_t)jj * ep.d + n ] : 0.0f;
+						if( ++jj == ep.rows_per_chunk ) jj = 0;
+					}
+				}
+#pragma unroll
+				for( int rr = 0; rr < 16; rr++ )
+				{
+					if( cb < ep.nchunks && j < ep.valid_per_chunk )
+						ep.out_f32[ ( (size_t)cb * ep.T + j ) * ep.ld + n ] = ptx::gelu_f16_semantics( w[ ( h + rr ) * STG_LD ] + b ) + pe[ rr ];
+					if( ++j == ep.rows_per_chunk ) { j = 0; cb++; }
+				}
 			}
 		}
 		else if constexpr( MODE == EPI_QKV )
@@ -246,20 +244,31 @@ namespace gemm
 			for( int rr = 0; rr < 32; rr++ )
 			{
 				if( mBase + rr < ep.M )
-					base[ ( ( (size_t)cb * ep.H + h ) * ep.T + t ) * 64 + e ] = __float2half_rn( w[ rr ] + b );
+					base[ ( ( (size_t)cb * ep.H + h ) * ep.T + t ) * 64 + e ] = __float2half_rn( w[ rr * STG_LD ] + b );
 				if( ++t == ep.T ) { t = 0; cb++; }
 			}
 		}
 		else if constexpr( MODE == EPI_BIAS_RESID )
 		{
-			// rs = the residual column, fetched by the caller one 32-column chunk ahead (loadResid): the 32 loads of a chunk are a
-			// full L2 round trip, and with only 4 epilogue warps that latency - not bandwidth - set the epilogue time (16 us per tile)
+			// the residual column 16 rows at a time ahead of the stores: issued one by one behind each store, its L2 round trips and
+			// not bandwidth would set the epilogue time
 			const float b = ep.bias[ n ];
 #pragma unroll
-			for( int rr = 0; rr < 32; rr++ )
+			for( int h = 0; h < 32; h += 16 )
 			{
-				const int m = mBase + rr;
-				if( m < ep.M ) ep.out_f32[ (size_t)m * ep.ld + n ] = w[ rr ] + b + rs[ rr ];
+				float rs[ 16 ];
+#pragma unroll
+				for( int rr = 0; rr < 16; rr++ )
+				{
+					const int m = mBase + h + rr;
+					rs[ rr ] = m < ep.M ? ep.resid[ (size_t)m * ep.ld + n ] : 0.0f;
+				}
+#pragma unroll
+				for( int rr = 0; rr < 16; rr++ )
+				{
+					const int m = mBase + h + rr;
+					if( m < ep.M ) ep.out_f32[ (size_t)m * ep.ld + n ] = w[ ( h + rr ) * STG_LD ] + b + rs[ rr ];
+				}
 			}
 		}
 		else if constexpr( MODE == EPI_BIAS_GELU_F16 )
@@ -269,7 +278,7 @@ namespace gemm
 			for( int rr = 0; rr < 32; rr++ )
 			{
 				const int m = mBase + rr;
-				if( m < ep.M ) ep.out_a[ (size_t)m * ep.ld + n ] = __float2half_rn( ptx::gelu_f16_semantics( w[ rr ] + b ) );
+				if( m < ep.M ) ep.out_a[ (size_t)m * ep.ld + n ] = __float2half_rn( ptx::gelu_f16_semantics( w[ rr * STG_LD ] + b ) );
 			}
 		}
 		else if constexpr( MODE == EPI_CROSSKV )
@@ -289,7 +298,7 @@ namespace gemm
 			for( int rr = 0; rr < 32; rr++ )
 			{
 				if( mBase + rr < ep.M )
-					base[ ( ( ( (size_t)l * ep.nchunks + cb ) * ep.H + h ) * ep.T + t ) * 64 + e ] = __float2half_rn( w[ rr ] * sc + b );
+					base[ ( ( ( (size_t)l * ep.nchunks + cb ) * ep.H + h ) * ep.T + t ) * 64 + e ] = __float2half_rn( w[ rr * STG_LD ] * sc + b );
 				if( ++t == ep.T ) { t = 0; cb++; }
 			}
 		}
@@ -302,33 +311,32 @@ namespace gemm
 		static constexpr int A_BYTES = BM * BK * 2;
 		static constexpr int B_BYTES = BN * BK * 2;
 		static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-		static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
-		static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;   // + barriers + alignment slack (the transpose tiles are static smem)
+		static constexpr int STG_OFFSET = STAGES * STAGE_BYTES;
+		static constexpr int STG_BYTES = 2 * 64 * STG_LD * 4;   // one 64 x 64 f32 staging tile per consumer warpgroup
+		static constexpr int BAR_OFFSET = STG_OFFSET + STG_BYTES;
+		static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;   // + barriers + alignment slack
+		static_assert( TOTAL <= 232448, "227 KB of shared memory per block on sm_90" );
 	};
 
 	template<int BN, int STAGES, int MODE, int AMODE>
-	__global__ void __launch_bounds__( 192, 1 )
+	__global__ void __launch_bounds__( 384, 1 )
 		gemm_tc_kernel( const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapB,
 			int M, int N, int K, int kTap, EpiParams ep )
 	{
 		using SL = SmemLayout<BN, STAGES>;
 		extern __shared__ uint8_t smem_raw[];
-		__shared__ float xposeTiles[ 4 ][ 32 * 33 ];   // one padded 32x32 transpose tile per epilogue warp (static: compiled to LDS/STS)
 		uint8_t* smem = reinterpret_cast<uint8_t*>( ( reinterpret_cast<uintptr_t>( smem_raw ) + 1023 ) & ~(uintptr_t)1023 );
 		uint64_t* bar_full = reinterpret_cast<uint64_t*>( smem + SL::BAR_OFFSET );
 		uint64_t* bar_empty = bar_full + STAGES;
-		uint64_t* bar_tfull = bar_empty + STAGES;
-		uint64_t* bar_tempty = bar_tfull + 2;
-		uint32_t* tmem_slot = reinterpret_cast<uint32_t*>( bar_tempty + 2 );
 
 		const int warp = threadIdx.x >> 5;
 		const int lane = threadIdx.x & 31;
+		const int wg = warp >> 2;
 
 		const int num_m = ( M + BM - 1 ) / BM;
 		const int num_n = ( N + BN - 1 ) / BN;
 		const int num_tiles = num_m * num_n;
 		const int num_kb = ( K + BK - 1 ) / BK;
-		constexpr uint32_t TMEM_COLS = 2 * BN;   // two accumulator stages (power of two: 256 or 512)
 
 		if( warp == 0 && lane == 0 )
 		{
@@ -338,29 +346,17 @@ namespace gemm
 			for( int s = 0; s < STAGES; s++ )
 			{
 				ptx::mbar_init( &bar_full[ s ], 1 );
-				ptx::mbar_init( &bar_empty[ s ], 1 );
-			}
-			for( int s = 0; s < 2; s++ )
-			{
-				ptx::mbar_init( &bar_tfull[ s ], 1 );
-				ptx::mbar_init( &bar_tempty[ s ], 4 );   // one arrive per epilogue warp
+				ptx::mbar_init( &bar_empty[ s ], 8 );   // one arrive per consumer warp
 			}
 			ptx::fence_barrier_init();
 		}
-		if( warp == 1 )
-		{
-			ptx::tmem_alloc( tmem_slot, TMEM_COLS );
-			ptx::tmem_relinquish();
-		}
-		ptx::tc_fence_before();
 		__syncthreads();
-		ptx::tc_fence_after();
-		const uint32_t tmem_base = *tmem_slot;
 
-		if( warp == 0 )
+		if( wg == 0 )
 		{
-			// ===== TMA producer =====
-			if( lane == 0 )
+			// ===== TMA producer (one thread); the warpgroup hands its registers to the consumers =====
+			asm volatile( "setmaxnreg.dec.sync.aligned.u32 40;" );
+			if( warp == 0 && lane == 0 )
 			{
 				int stage = 0;
 				uint32_t phase = 0;
@@ -395,122 +391,95 @@ namespace gemm
 					}
 				}
 			}
-			__syncwarp();
-		}
-		else if( warp == 1 )
-		{
-			// ===== MMA issuer =====
-			if( lane == 0 )
-			{
-				constexpr uint32_t idesc = ptx::umma_idesc_f16( BM, BN );
-				int stage = 0;
-				uint32_t phase = 0;
-				int as = 0;
-				uint32_t aphase = 0;
-				for( int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x )
-				{
-					ptx::mbar_wait( &bar_tempty[ as ], aphase ^ 1 );
-					ptx::tc_fence_after();
-					const uint32_t tmem_d = tmem_base + (uint32_t)( as * BN );
-					for( int kb = 0; kb < num_kb; kb++ )
-					{
-						ptx::mbar_wait( &bar_full[ stage ], phase );
-						ptx::tc_fence_after();
-						const uint32_t sa = ptx::smem_u32( smem + stage * SL::STAGE_BYTES );
-						const uint64_t da = ptx::umma_desc_sw128( sa );
-						const uint64_t db = ptx::umma_desc_sw128( sa + SL::A_BYTES );
-#pragma unroll
-						for( int k = 0; k < BK / 16; k++ )
-						{
-							// advance 16 f16 = 32 bytes along K inside the 128-byte swizzle row: +2 in the (addr >> 4) field
-							ptx::umma_f16( tmem_d, da + (uint64_t)( k * 2 ), db + (uint64_t)( k * 2 ), idesc, ( kb | k ) != 0 ? 1u : 0u );
-						}
-						ptx::umma_commit( &bar_empty[ stage ] );
-						if( kb == num_kb - 1 )
-							ptx::umma_commit( &bar_tfull[ as ] );
-						if( ++stage == STAGES ) { stage = 0; phase ^= 1; }
-					}
-					as ^= 1;
-					if( as == 0 ) aphase ^= 1;
-				}
-			}
-			__syncwarp();
-		}
-		else
-		{
-			// ===== epilogue warps =====
-			const int q = warp & 3;   // TMEM lane quadrant accessible to this warp
-			int as = 0;
-			uint32_t aphase = 0;
-			for( int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x )
-			{
-				const int m0 = ( tile / num_n ) * BM;
-				const int n0 = ( tile % num_n ) * BN;
-				// the residual of the first column chunk does not depend on the accumulator: request it before waiting for the MMAs
-				float rsNext[ 32 ];
-				if constexpr( MODE == EPI_BIAS_RESID ) loadResid( ep, m0 + q * 32, n0 + lane, rsNext );
-				ptx::mbar_wait( &bar_tfull[ as ], aphase );
-				ptx::tc_fence_after();
-				const int m = m0 + q * 32 + lane;
-				const uint32_t taddr = tmem_base + ( (uint32_t)( q * 32 ) << 16 ) + (uint32_t)( as * BN );
-				float* xpose = xposeTiles[ warp - 2 ];
-#pragma unroll 1
-				for( int c = 0; c < BN / 32; c++ )
-				{
-					uint32_t r[ 32 ];
-					ptx::tmem_ld_32x32( taddr + (uint32_t)( c * 32 ), r );
-					ptx::tmem_ld_wait();
-					const int nc = n0 + c * 32;
-					// f32 outputs go through the transpose (measured: out-projection 99 -> 79 us); f16 outputs keep the row-per-thread
-					// layout with 16-byte stores — 2-byte scalar stores, even though contiguous across the warp, were measured 2x slower
-					// (fc1 144 -> 269 us), and the V^T band of the QKV GEMM is stored transposed, for which row-per-thread is the coalesced layout
-					constexpr bool rowLayout = ( MODE == EPI_QKV ) || ( MODE == EPI_CONV1 ) || ( MODE == EPI_BIAS_GELU_F16 ) || ( MODE == EPI_CROSSKV );
-					if( rowLayout )
-					{
-						float v[ 32 ];
-#pragma unroll
-						for( int i = 0; i < 32; i++ )
-							v[ i ] = __uint_as_float( r[ i ] );
-						epilogue<MODE>( ep, m, nc, v );
-					}
-					else
-					{
-#pragma unroll
-						for( int i = 0; i < 32; i++ )
-							xpose[ lane * 33 + i ] = __uint_as_float( r[ i ] );
-						__syncwarp();
-						float w[ 32 ];
-#pragma unroll
-						for( int rr = 0; rr < 32; rr++ )
-							w[ rr ] = xpose[ rr * 33 + lane ];
-						__syncwarp();
-						if constexpr( MODE == EPI_BIAS_RESID )
-						{
-							float rs[ 32 ];
-#pragma unroll
-							for( int rr = 0; rr < 32; rr++ ) rs[ rr ] = rsNext[ rr ];
-							if( c + 1 < BN / 32 ) loadResid( ep, m0 + q * 32, nc + 32 + lane, rsNext );   // next chunk's residual while this one is stored
-							epilogueT<MODE>( ep, m0 + q * 32, nc + lane, w, rs );
-						}
-						else
-							epilogueT<MODE>( ep, m0 + q * 32, nc + lane, w );
-					}
-				}
-				ptx::tc_fence_before();
-				__syncwarp();
-				if( lane == 0 )
-					ptx::mbar_arrive( &bar_tempty[ as ] );
-				as ^= 1;
-				if( as == 0 ) aphase ^= 1;
-			}
+			return;
 		}
 
-		ptx::tc_fence_before();
-		__syncthreads();
-		if( warp == 1 )
+		// ===== consumer warpgroups: warpgroup c owns rows [64c, 64c + 64) of the 128-row tile =====
+		asm volatile( "setmaxnreg.inc.sync.aligned.u32 232;" );
+		const int c = wg - 1;
+		const int wq = warp & 3;   // warp inside the warpgroup
+		float* stg = reinterpret_cast<float*>( smem + SL::STG_OFFSET ) + c * 64 * STG_LD;
+		int stage = 0;
+		uint32_t phase = 0;
+		for( int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x )
 		{
-			ptx::tc_fence_after();
-			ptx::tmem_dealloc( tmem_base, TMEM_COLS );
+			const int m0 = ( tile / num_n ) * BM;
+			const int n0 = ( tile % num_n ) * BN;
+			float acc[ BN / 2 ];
+			int prev = -1;
+			for( int kb = 0; kb < num_kb; kb++ )
+			{
+				ptx::mbar_wait( &bar_full[ stage ], phase );
+				const uint32_t sa = ptx::smem_u32( smem + stage * SL::STAGE_BYTES );
+				const uint64_t da = ptx::gmma_desc_sw128( sa + (uint32_t)( c * 64 * 128 ) );
+				const uint64_t db = ptx::gmma_desc_sw128( sa + SL::A_BYTES );
+				ptx::fence_regs<BN / 2>( acc );
+				ptx::wgmma_fence();
+#pragma unroll
+				for( int k = 0; k < BK / 16; k++ )
+				{
+					if constexpr( BN == 256 )
+						ptx::wgmma_m64n256k16_ss( acc, da + (uint64_t)( k * 2 ), db + (uint64_t)( k * 2 ), ( kb | k ) != 0 ? 1u : 0u );
+					else
+						ptx::wgmma_m64n128k16_ss( acc, da + (uint64_t)( k * 2 ), db + (uint64_t)( k * 2 ), ( kb | k ) != 0 ? 1u : 0u );
+				}
+				ptx::wgmma_commit();
+				ptx::fence_regs<BN / 2>( acc );
+				// one k-block in flight: the previous one has finished reading its stage
+				ptx::wgmma_wait<1>();
+				if( prev >= 0 )
+				{
+					__syncwarp();
+					if( lane == 0 ) ptx::mbar_arrive( &bar_empty[ prev ] );
+				}
+				prev = stage;
+				if( ++stage == STAGES ) { stage = 0; phase ^= 1; }
+			}
+			ptx::wgmma_wait<0>();
+			ptx::fence_regs<BN / 2>( acc );
+			__syncwarp();
+			if( lane == 0 ) ptx::mbar_arrive( &bar_empty[ prev ] );
+
+			// epilogue: 64 columns at a time through the staging tile; warp wq then handles the 32 x 32 chunk
+			// (rows 32 * (wq >> 1), columns 32 * (wq & 1)) of it with the epilogue of the old row- / column-per-thread layouts
+			const int fr = wq * 16 + ( lane >> 2 );
+			const int fc = ( lane & 3 ) * 2;
+			const int mBase = m0 + c * 64 + ( wq >> 1 ) * 32;
+			const int cOff = ( wq & 1 ) * 32;
+#pragma unroll
+			for( int piece = 0; piece < BN / 64; piece++ )
+			{
+				ptx::named_bar_sync( 1 + c, 128 );   // the previous piece has been read
+#pragma unroll
+				for( int j = 0; j < 8; j++ )
+				{
+					const float* a = acc + ( piece * 8 + j ) * 4;
+					*reinterpret_cast<float2*>( stg + fr * STG_LD + j * 8 + fc ) = make_float2( a[ 0 ], a[ 1 ] );
+					*reinterpret_cast<float2*>( stg + ( fr + 8 ) * STG_LD + j * 8 + fc ) = make_float2( a[ 2 ], a[ 3 ] );
+				}
+				ptx::named_bar_sync( 1 + c, 128 );
+				const int nc = n0 + piece * 64 + cOff;
+				// f32 outputs are read column-per-thread; f16 outputs keep the row-per-thread layout with 16-byte stores (2-byte scalar
+				// stores, even though contiguous across the warp, are slower), and the V^T band of the QKV GEMM is stored transposed,
+				// for which row-per-thread is the coalesced layout
+				constexpr bool rowLayout = ( MODE == EPI_QKV ) || ( MODE == EPI_CONV1 ) || ( MODE == EPI_BIAS_GELU_F16 ) || ( MODE == EPI_CROSSKV );
+				if constexpr( rowLayout )
+				{
+					float v[ 32 ];
+					const float* src = stg + ( ( wq >> 1 ) * 32 + lane ) * STG_LD + cOff;
+#pragma unroll
+					for( int i = 0; i < 8; i++ )
+					{
+						const float4 t = reinterpret_cast<const float4*>( src )[ i ];
+						v[ i * 4 + 0 ] = t.x; v[ i * 4 + 1 ] = t.y; v[ i * 4 + 2 ] = t.z; v[ i * 4 + 3 ] = t.w;
+					}
+					epilogue<MODE>( ep, mBase + lane, nc, v );
+				}
+				else
+				{
+					epilogueT<MODE>( ep, mBase, nc + lane, stg + ( ( wq >> 1 ) * 32 ) * STG_LD + cOff + lane );
+				}
+			}
 		}
 	}
 
@@ -564,15 +533,15 @@ namespace gemm
 		const int num_tiles = ( ( L.M + BM - 1 ) / BM ) * ( ( L.N + BN - 1 ) / BN );
 		const int grid = num_tiles < numSMs ? num_tiles : numSMs;
 		if( grid <= 0 ) return cudaSuccess;
-		kfn<<<grid, 192, SL::TOTAL, stream>>>( L.mapA, L.mapA2, L.mapB, L.M, L.N, L.K, L.kTap, L.ep );
+		kfn<<<grid, 384, SL::TOTAL, stream>>>( L.mapA, L.mapA2, L.mapB, L.M, L.N, L.K, L.kTap, L.ep );
 		return cudaGetLastError();
 	}
 
 	template<int MODE, int AMODE>
 	static cudaError_t launchBN( const Launch& L, int bn, int numSMs, cudaStream_t stream )
 	{
-		if( bn == 256 ) return launchT<256, 4, MODE, AMODE>( L, numSMs, stream );
-		return launchT<128, 6, MODE, AMODE>( L, numSMs, stream );
+		if( bn == 256 ) return launchT<256, 3, MODE, AMODE>( L, numSMs, stream );
+		return launchT<128, 5, MODE, AMODE>( L, numSMs, stream );
 	}
 
 	cudaError_t launch( const Launch& L, EpiMode epi, AMode amode, int bn, int numSMs, cudaStream_t stream )

@@ -1,15 +1,15 @@
-// Persistent, warp-specialised tcgen05 GEMM for sm_100a:  D[M,N] = A[M,K] * B[N,K]^T  (both operands f16, K-major; f32 accumulate)
+// Persistent, warp-specialised wgmma GEMM for sm_90a:  D[M,N] = A[M,K] * B[N,K]^T  (both operands f16, K-major; f32 accumulate)
 //
 // Replaces the reference's mulMatTiled.hlsl (43 % of its GPU time, ComputeShaders/mulMatTiled.hlsl:203-274, host call
 // Whisper/ML/MlContext.cpp:132-147) and the ggml CPU path ggml_compute_forward_mul_mat_f16_f32 (Whisper/source/ggml.c:4447-4749),
-// whose arithmetic — activation rounded to f16, f16 x f16 products, f32 accumulation — is exactly what kind::f16 does.
+// whose arithmetic — activation rounded to f16, f16 x f16 products, f32 accumulation — is exactly what wgmma .f32.f16.f16 does.
 //
-//   warp 0      : TMA producer   (cp.async.bulk.tensor 2D, 128B swizzle, mbarrier complete_tx)
-//   warp 1      : MMA issuer     (one thread: tcgen05.mma cta_group::1 kind::f16, M=128, N=BN, K=16; tcgen05.commit)
-//   warps 2..5  : epilogue       (tcgen05.ld 32x32b.x32 -> registers -> fused epilogue -> global)
+//   warpgroup 0    : TMA producer   (one thread: cp.async.bulk.tensor 2D, 128B swizzle, mbarrier complete_tx)
+//   warpgroups 1-2 : consumers      (wgmma.mma_async m64nBNk16, rows [0,64) and [64,128) of the 128 x BN tile, accumulators in
+//                                    registers; then the fused epilogue through a 64 x 64 shared-memory staging tile)
 //
-// Three pipelines: smem full/empty (TMA <-> MMA), TMEM full/empty (MMA <-> epilogue, two accumulator stages so the
-// epilogue of tile i overlaps the main loop of tile i+1), and a static persistent tile schedule (grid = #SMs).
+// Pipeline: smem full/empty mbarriers between the producer and the consumers (one k-block of wgmma kept in flight), and a static
+// persistent tile schedule (grid = #SMs), so the producer already streams the next tile while the consumers run the epilogue.
 //
 // The fused epilogues are the reference's element-wise shaders folded in: addRepeat / addRepeatScale / addRepeatGelu /
 // addRepeatEx / copyConvert / copyTranspose (SURVEY.md §2.2), writing head-major f16 Q/K, transposed V and the f16

@@ -668,8 +668,8 @@ namespace kern
 	// after thread 0 has run the exact algorithm over the first TIE_PRE elements, every later element that is not above the root
 	// reached there (T1) can be dropped without changing a single heap operation: all warps filter their contiguous region of the row
 	// against T1 (coalesced loads, ballot, survivors appended in index order to `scratch`), and thread 0 replays the exact algorithm
-	// over the survivors only.  A row whose top probability is shared costs ~10 us this way instead of ~110 us on one thread
-	// (degenerate rows tie at every step: that was 11 % of a decoder step).  Called by every thread of the CTA; the result is valid
+	// over the survivors only.  A row whose top probability is shared is far cheaper this way than on one thread
+	// (degenerate rows tie at every step).  Called by every thread of the CTA; the result is valid
 	// in thread 0.  scratch: nv + 32 * warps ints.
 	constexpr int TIE_PRE = 1024;
 	struct TieShared
@@ -845,7 +845,7 @@ namespace kern
 		const int nv = a.nVocab;
 		const float* lg = a.logits + (size_t)b * nv;
 		float* gpr = a.probs + (size_t)b * nv;
-		// the row lives in shared memory when it fits (207 KB for 51865 tokens): seven passes over L2 cost 65 us, over smem ~15 us
+		// the row lives in shared memory when it fits (207 KB for 51865 tokens): its seven passes then read shared memory instead of L2
 		extern __shared__ float sampleRow[];
 		float* pr = a.rowInSmem ? sampleRow : gpr;
 		const bool forceTs = a.dForceTs && a.dForceTs[ 0 ] != 0;
@@ -920,7 +920,7 @@ namespace kern
 
 	// The same sampler with one vocabulary row spread over a cluster of SC_CL CTAs: every CTA keeps its slice of the row in shared
 	// memory, the three row-wide reductions go through distributed shared memory (each CTA publishes its partial, cluster barrier,
-	// everybody combines the SC_CL partials in rank order).  8 rows on 8 SMs left 140 SMs idle for 37 us per token step.
+	// everybody combines the SC_CL partials in rank order).  8 rows on 8 SMs leave the other SMs idle.
 	struct ClusterPart
 	{
 		float mx, maxTx;
@@ -1089,7 +1089,7 @@ namespace kern
 	cudaError_t sampleGreedy( const SampleArgs& a, cudaStream_t s )
 	{
 		SampleArgs sa = a;
-		// cluster size: 4 by default (measured 157.0 -> 155.4 ms per 100 tokens against the single-CTA kernel); WSP_SAMPLER_CLUSTER=0|4|8 for A/B runs
+		// cluster size: 4 by default; WSP_SAMPLER_CLUSTER=0|4|8 for A/B runs
 		static const int clusterSize = []() { const char* e = getenv( "WSP_SAMPLER_CLUSTER" ); return e ? atoi( e ) : 4; }();
 		if( ( clusterSize == 4 || clusterSize == 8 ) && a.nVocab >= 4096 )
 		{

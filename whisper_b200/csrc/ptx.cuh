@@ -1,8 +1,7 @@
-// Thin inline-PTX layer for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and
-// the UMMA shared-memory + instruction descriptors.  Everything here is hand-written for B200; there is no other target.
+// Thin inline-PTX layer for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / mma_async / commit / wait) and the
+// wgmma shared-memory descriptor.  Everything here is hand-written for H100; there is no other target.
 //
-// Descriptor bit layouts were cross-checked against the CUTLASS headers vendored in this image
-// (cute/arch/mma_sm100_desc.hpp: SmemDescriptor, InstrDescriptor) — the layouts are hardware facts, the code is ours.
+// The descriptor bit layout follows the PTX ISA's "Matrix Descriptor Format" for wgmma — the layouts are hardware facts.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -82,86 +81,72 @@ namespace ptx
 	}
 
 	// ---------------------------------------------------------------------------------------------
-	// tcgen05: tensor memory management
-	__device__ __forceinline__ void tmem_alloc( uint32_t* dst_smem, uint32_t ncols )
+	// wgmma: warpgroup MMA, f16 inputs, f32 accumulators in registers.  All 128 threads of a warpgroup issue each instruction.
+	//
+	// Accumulator layout of m64nNk16 (per warp w of the warpgroup, lane l, q = l & 3): d[4j + 0/1] = row 16w + l/4, columns
+	// 8j + 2q + 0/1;  d[4j + 2/3] = row 16w + l/4 + 8, same columns.  A register A fragment of m64k16 has the same shape:
+	// {a0, a1, a2, a3} = (row, k 2q..2q+1), (row + 8, k 2q..2q+1), (row, k 2q+8..2q+9), (row + 8, k 2q+8..2q+9), two f16 each.
+	__device__ __forceinline__ void wgmma_fence() { asm volatile( "wgmma.fence.sync.aligned;" ::: "memory" ); }
+	__device__ __forceinline__ void wgmma_commit() { asm volatile( "wgmma.commit_group.sync.aligned;" ::: "memory" ); }
+	template<int N>
+	__device__ __forceinline__ void wgmma_wait() { asm volatile( "wgmma.wait_group.sync.aligned %0;" ::"n"( N ) : "memory" ); }
+	// keep the compiler from moving accumulator reads / writes across an in-flight wgmma
+	template<int N>
+	__device__ __forceinline__ void fence_regs( float* d )
 	{
-		asm volatile( "tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"( smem_u32( dst_smem ) ), "r"( ncols ) : "memory" );
-	}
-	__device__ __forceinline__ void tmem_relinquish() { asm volatile( "tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory" ); }
-	__device__ __forceinline__ void tmem_dealloc( uint32_t taddr, uint32_t ncols )
-	{
-		asm volatile( "tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"( taddr ), "r"( ncols ) : "memory" );
-	}
-	__device__ __forceinline__ void tc_fence_before() { asm volatile( "tcgen05.fence::before_thread_sync;" ::: "memory" ); }
-	__device__ __forceinline__ void tc_fence_after() { asm volatile( "tcgen05.fence::after_thread_sync;" ::: "memory" ); }
-
-	// D[tmem] (+)= A[smem desc] * B[smem desc], f16 inputs, f32 accumulate.  One thread issues for the CTA.
-	__device__ __forceinline__ void umma_f16( uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate )
-	{
-		asm volatile(
-			"{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-			"tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-			::"r"( tmem_d ), "l"( desc_a ), "l"( desc_b ), "r"( idesc ), "r"( accumulate )
-			: "memory" );
-	}
-	// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-	// (implies tcgen05.fence::before_thread_sync)
-	__device__ __forceinline__ void umma_commit( uint64_t* bar )
-	{
-		asm volatile( "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"( smem_u32( bar ) ) : "memory" );
+#pragma unroll
+		for( int i = 0; i < N; i++ ) asm volatile( "" : "+f"( d[ i ] )::"memory" );
 	}
 
-	// TMEM -> registers: 32 lanes (this warp's quadrant) x 32 consecutive 32-bit columns; thread i gets lane i.
-	__device__ __forceinline__ void tmem_ld_32x32( uint32_t taddr, uint32_t* r )
+	// D (+)= A * B^T, A = [64][16] and B = [N][16] K-major tiles in shared memory (descriptors below)
+	__device__ __forceinline__ void wgmma_m64n128k16_ss( float* d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate )
 	{
 		asm volatile(
-			"tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-			"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-			"%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-			: "=r"( r[ 0 ] ), "=r"( r[ 1 ] ), "=r"( r[ 2 ] ), "=r"( r[ 3 ] ), "=r"( r[ 4 ] ), "=r"( r[ 5 ] ), "=r"( r[ 6 ] ), "=r"( r[ 7 ] ),
-			  "=r"( r[ 8 ] ), "=r"( r[ 9 ] ), "=r"( r[ 10 ] ), "=r"( r[ 11 ] ), "=r"( r[ 12 ] ), "=r"( r[ 13 ] ), "=r"( r[ 14 ] ), "=r"( r[ 15 ] ),
-			  "=r"( r[ 16 ] ), "=r"( r[ 17 ] ), "=r"( r[ 18 ] ), "=r"( r[ 19 ] ), "=r"( r[ 20 ] ), "=r"( r[ 21 ] ), "=r"( r[ 22 ] ), "=r"( r[ 23 ] ),
-			  "=r"( r[ 24 ] ), "=r"( r[ 25 ] ), "=r"( r[ 26 ] ), "=r"( r[ 27 ] ), "=r"( r[ 28 ] ), "=r"( r[ 29 ] ), "=r"( r[ 30 ] ), "=r"( r[ 31 ] )
-			: "r"( taddr )
-			: "memory" );
+			"{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+			"wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+			"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+			"%64, %65, p, 1, 1, 0, 0;\n\t}\n"
+			: "+f"( d[ 0 ] ), "+f"( d[ 1 ] ), "+f"( d[ 2 ] ), "+f"( d[ 3 ] ), "+f"( d[ 4 ] ), "+f"( d[ 5 ] ), "+f"( d[ 6 ] ), "+f"( d[ 7 ] ), "+f"( d[ 8 ] ), "+f"( d[ 9 ] ), "+f"( d[ 10 ] ), "+f"( d[ 11 ] ), "+f"( d[ 12 ] ), "+f"( d[ 13 ] ), "+f"( d[ 14 ] ), "+f"( d[ 15 ] ), "+f"( d[ 16 ] ), "+f"( d[ 17 ] ), "+f"( d[ 18 ] ), "+f"( d[ 19 ] ), "+f"( d[ 20 ] ), "+f"( d[ 21 ] ), "+f"( d[ 22 ] ), "+f"( d[ 23 ] ), "+f"( d[ 24 ] ), "+f"( d[ 25 ] ), "+f"( d[ 26 ] ), "+f"( d[ 27 ] ), "+f"( d[ 28 ] ), "+f"( d[ 29 ] ), "+f"( d[ 30 ] ), "+f"( d[ 31 ] ), "+f"( d[ 32 ] ), "+f"( d[ 33 ] ), "+f"( d[ 34 ] ), "+f"( d[ 35 ] ), "+f"( d[ 36 ] ), "+f"( d[ 37 ] ), "+f"( d[ 38 ] ), "+f"( d[ 39 ] ), "+f"( d[ 40 ] ), "+f"( d[ 41 ] ), "+f"( d[ 42 ] ), "+f"( d[ 43 ] ), "+f"( d[ 44 ] ), "+f"( d[ 45 ] ), "+f"( d[ 46 ] ), "+f"( d[ 47 ] ), "+f"( d[ 48 ] ), "+f"( d[ 49 ] ), "+f"( d[ 50 ] ), "+f"( d[ 51 ] ), "+f"( d[ 52 ] ), "+f"( d[ 53 ] ), "+f"( d[ 54 ] ), "+f"( d[ 55 ] ), "+f"( d[ 56 ] ), "+f"( d[ 57 ] ), "+f"( d[ 58 ] ), "+f"( d[ 59 ] ), "+f"( d[ 60 ] ), "+f"( d[ 61 ] ), "+f"( d[ 62 ] ), "+f"( d[ 63 ] )
+			: "l"( desc_a ), "l"( desc_b ), "r"( accumulate ) );
 	}
-	__device__ __forceinline__ void tmem_ld_wait() { asm volatile( "tcgen05.wait::ld.sync.aligned;" ::: "memory" ); }
-	// registers -> TMEM, the mirror image of tmem_ld_32x32
-	__device__ __forceinline__ void tmem_st_32x32( uint32_t taddr, const uint32_t* r )
+	__device__ __forceinline__ void wgmma_m64n256k16_ss( float* d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate )
 	{
 		asm volatile(
-			"tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-			"{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-			"%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-			:
-			: "r"( taddr ), "r"( r[ 0 ] ), "r"( r[ 1 ] ), "r"( r[ 2 ] ), "r"( r[ 3 ] ), "r"( r[ 4 ] ), "r"( r[ 5 ] ), "r"( r[ 6 ] ), "r"( r[ 7 ] ),
-			  "r"( r[ 8 ] ), "r"( r[ 9 ] ), "r"( r[ 10 ] ), "r"( r[ 11 ] ), "r"( r[ 12 ] ), "r"( r[ 13 ] ), "r"( r[ 14 ] ), "r"( r[ 15 ] ),
-			  "r"( r[ 16 ] ), "r"( r[ 17 ] ), "r"( r[ 18 ] ), "r"( r[ 19 ] ), "r"( r[ 20 ] ), "r"( r[ 21 ] ), "r"( r[ 22 ] ), "r"( r[ 23 ] ),
-			  "r"( r[ 24 ] ), "r"( r[ 25 ] ), "r"( r[ 26 ] ), "r"( r[ 27 ] ), "r"( r[ 28 ] ), "r"( r[ 29 ] ), "r"( r[ 30 ] ), "r"( r[ 31 ] )
-			: "memory" );
+			"{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+			"wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+			"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+			"%128, %129, p, 1, 1, 0, 0;\n\t}\n"
+			: "+f"( d[ 0 ] ), "+f"( d[ 1 ] ), "+f"( d[ 2 ] ), "+f"( d[ 3 ] ), "+f"( d[ 4 ] ), "+f"( d[ 5 ] ), "+f"( d[ 6 ] ), "+f"( d[ 7 ] ), "+f"( d[ 8 ] ), "+f"( d[ 9 ] ), "+f"( d[ 10 ] ), "+f"( d[ 11 ] ), "+f"( d[ 12 ] ), "+f"( d[ 13 ] ), "+f"( d[ 14 ] ), "+f"( d[ 15 ] ), "+f"( d[ 16 ] ), "+f"( d[ 17 ] ), "+f"( d[ 18 ] ), "+f"( d[ 19 ] ), "+f"( d[ 20 ] ), "+f"( d[ 21 ] ), "+f"( d[ 22 ] ), "+f"( d[ 23 ] ), "+f"( d[ 24 ] ), "+f"( d[ 25 ] ), "+f"( d[ 26 ] ), "+f"( d[ 27 ] ), "+f"( d[ 28 ] ), "+f"( d[ 29 ] ), "+f"( d[ 30 ] ), "+f"( d[ 31 ] ), "+f"( d[ 32 ] ), "+f"( d[ 33 ] ), "+f"( d[ 34 ] ), "+f"( d[ 35 ] ), "+f"( d[ 36 ] ), "+f"( d[ 37 ] ), "+f"( d[ 38 ] ), "+f"( d[ 39 ] ), "+f"( d[ 40 ] ), "+f"( d[ 41 ] ), "+f"( d[ 42 ] ), "+f"( d[ 43 ] ), "+f"( d[ 44 ] ), "+f"( d[ 45 ] ), "+f"( d[ 46 ] ), "+f"( d[ 47 ] ), "+f"( d[ 48 ] ), "+f"( d[ 49 ] ), "+f"( d[ 50 ] ), "+f"( d[ 51 ] ), "+f"( d[ 52 ] ), "+f"( d[ 53 ] ), "+f"( d[ 54 ] ), "+f"( d[ 55 ] ), "+f"( d[ 56 ] ), "+f"( d[ 57 ] ), "+f"( d[ 58 ] ), "+f"( d[ 59 ] ), "+f"( d[ 60 ] ), "+f"( d[ 61 ] ), "+f"( d[ 62 ] ), "+f"( d[ 63 ] ), "+f"( d[ 64 ] ), "+f"( d[ 65 ] ), "+f"( d[ 66 ] ), "+f"( d[ 67 ] ), "+f"( d[ 68 ] ), "+f"( d[ 69 ] ), "+f"( d[ 70 ] ), "+f"( d[ 71 ] ), "+f"( d[ 72 ] ), "+f"( d[ 73 ] ), "+f"( d[ 74 ] ), "+f"( d[ 75 ] ), "+f"( d[ 76 ] ), "+f"( d[ 77 ] ), "+f"( d[ 78 ] ), "+f"( d[ 79 ] ), "+f"( d[ 80 ] ), "+f"( d[ 81 ] ), "+f"( d[ 82 ] ), "+f"( d[ 83 ] ), "+f"( d[ 84 ] ), "+f"( d[ 85 ] ), "+f"( d[ 86 ] ), "+f"( d[ 87 ] ), "+f"( d[ 88 ] ), "+f"( d[ 89 ] ), "+f"( d[ 90 ] ), "+f"( d[ 91 ] ), "+f"( d[ 92 ] ), "+f"( d[ 93 ] ), "+f"( d[ 94 ] ), "+f"( d[ 95 ] ), "+f"( d[ 96 ] ), "+f"( d[ 97 ] ), "+f"( d[ 98 ] ), "+f"( d[ 99 ] ), "+f"( d[ 100 ] ), "+f"( d[ 101 ] ), "+f"( d[ 102 ] ), "+f"( d[ 103 ] ), "+f"( d[ 104 ] ), "+f"( d[ 105 ] ), "+f"( d[ 106 ] ), "+f"( d[ 107 ] ), "+f"( d[ 108 ] ), "+f"( d[ 109 ] ), "+f"( d[ 110 ] ), "+f"( d[ 111 ] ), "+f"( d[ 112 ] ), "+f"( d[ 113 ] ), "+f"( d[ 114 ] ), "+f"( d[ 115 ] ), "+f"( d[ 116 ] ), "+f"( d[ 117 ] ), "+f"( d[ 118 ] ), "+f"( d[ 119 ] ), "+f"( d[ 120 ] ), "+f"( d[ 121 ] ), "+f"( d[ 122 ] ), "+f"( d[ 123 ] ), "+f"( d[ 124 ] ), "+f"( d[ 125 ] ), "+f"( d[ 126 ] ), "+f"( d[ 127 ] )
+			: "l"( desc_a ), "l"( desc_b ), "r"( accumulate ) );
 	}
-	__device__ __forceinline__ void tmem_st_wait() { asm volatile( "tcgen05.wait::st.sync.aligned;" ::: "memory" ); }
+	// D (+)= A * B^T with A = [64][16] in registers (the fragment above), B = [64][16] K-major in shared memory
+	__device__ __forceinline__ void wgmma_m64n64k16_rs( float* d, const uint32_t* a, uint64_t desc_b, uint32_t accumulate )
+	{
+		asm volatile(
+			"{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+			"wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+			"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+			"{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}\n"
+			: "+f"( d[ 0 ] ), "+f"( d[ 1 ] ), "+f"( d[ 2 ] ), "+f"( d[ 3 ] ), "+f"( d[ 4 ] ), "+f"( d[ 5 ] ), "+f"( d[ 6 ] ), "+f"( d[ 7 ] ), "+f"( d[ 8 ] ), "+f"( d[ 9 ] ), "+f"( d[ 10 ] ), "+f"( d[ 11 ] ), "+f"( d[ 12 ] ), "+f"( d[ 13 ] ), "+f"( d[ 14 ] ), "+f"( d[ 15 ] ), "+f"( d[ 16 ] ), "+f"( d[ 17 ] ), "+f"( d[ 18 ] ), "+f"( d[ 19 ] ), "+f"( d[ 20 ] ), "+f"( d[ 21 ] ), "+f"( d[ 22 ] ), "+f"( d[ 23 ] ), "+f"( d[ 24 ] ), "+f"( d[ 25 ] ), "+f"( d[ 26 ] ), "+f"( d[ 27 ] ), "+f"( d[ 28 ] ), "+f"( d[ 29 ] ), "+f"( d[ 30 ] ), "+f"( d[ 31 ] )
+			: "r"( a[ 0 ] ), "r"( a[ 1 ] ), "r"( a[ 2 ] ), "r"( a[ 3 ] ), "l"( desc_b ), "r"( accumulate ) );
+	}
+
+	// Named barrier over `count` threads (ids 1..15; 0 is __syncthreads)
+	__device__ __forceinline__ void named_bar_sync( int id, int count ) { asm volatile( "bar.sync %0, %1;" ::"r"( id ), "r"( count ) : "memory" ); }
 
 	// ---------------------------------------------------------------------------------------------
-	// UMMA descriptors
-	//
-	// Shared-memory matrix descriptor for a K-major operand tile stored as rows of 64 f16 (128 bytes) with the
-	// 128-byte swizzle TMA writes (CU_TENSOR_MAP_SWIZZLE_128B): 8-row groups are 1024 bytes apart (SBO), LBO is
-	// unused for swizzled K-major (encoded 1), version = 1 (sm_100), layout type 2 = SWIZZLE_128B.
-	__device__ __forceinline__ uint64_t umma_desc_sw128( uint32_t smem_addr )
+	// Shared-memory matrix descriptor (sm_90 wgmma) for a K-major operand tile stored as rows of 64 f16 (128 bytes) with the
+	// 128-byte swizzle TMA writes (CU_TENSOR_MAP_SWIZZLE_128B): 8-row groups are 1024 bytes apart (stride byte offset), the
+	// leading byte offset is unused for swizzled K-major (encoded 1), layout type 1 = SWIZZLE_128B.  Tiles start 1024-aligned;
+	// the k-th 16-element slice of a row starts 32 bytes further: +2 in the (address >> 4) field.
+	__device__ __forceinline__ uint64_t gmma_desc_sw128( uint32_t smem_addr )
 	{
 		uint64_t d = 0;
 		d |= (uint64_t)( ( smem_addr & 0x3FFFF ) >> 4 );         // [0,14)  start address >> 4
 		d |= (uint64_t)1 << 16;                                   // [16,30) leading byte offset >> 4 (ignored)
 		d |= (uint64_t)( 1024 >> 4 ) << 32;                       // [32,46) stride byte offset >> 4
-		d |= (uint64_t)1 << 46;                                   // [46,48) descriptor version (Blackwell)
-		d |= (uint64_t)2 << 61;                                   // [61,64) SWIZZLE_128B
+		d |= (uint64_t)1 << 62;                                   // [62,64) SWIZZLE_128B
 		return d;
-	}
-	// Instruction descriptor, kind::f16: A,B = f16 (format 0), D = f32 (1), both operands K-major, dense.
-	__host__ __device__ constexpr uint32_t umma_idesc_f16( int M, int N )
-	{
-		return ( 1u << 4 ) | ( (uint32_t)( N >> 3 ) << 17 ) | ( (uint32_t)( M >> 4 ) << 24 );
 	}
 
 	// Programmatic dependent launch: let the next kernel of the stream start its prologue (weight / KV prefetch) while this one runs,

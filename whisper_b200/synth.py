@@ -11,6 +11,7 @@ from __future__ import annotations
 
 import os
 import struct
+import tempfile
 from dataclasses import dataclass
 
 import numpy as np
@@ -411,7 +412,8 @@ def write_script_model(path: str, base: str, seed: int = 1234, stage: int = 2, c
 
 def model_path(name: str, seed: int = 1234, cache_dir: str | None = None) -> str:
     """Return (creating on first use) the cached synthetic model file for `name`."""
-    cache_dir = cache_dir or os.environ.get("WSP_MODEL_CACHE", "/tmp/wsp_models")
+    # one cache per user: a directory another account created first is not writable
+    cache_dir = cache_dir or os.environ.get("WSP_MODEL_CACHE") or os.path.join(tempfile.gettempdir(), "wsp_models-%d" % os.getuid())
     os.makedirs(cache_dir, exist_ok=True)
     p = os.path.join(cache_dir, "ggml-%s-synth%d%s.bin" % (name, seed, "-r2" if name.endswith(("-sc", "-sc1")) else ""))
     if not os.path.exists(p):
