@@ -12,6 +12,7 @@
  *   wsp_pcm_to_mel_window     Whisper/Whisper/MelStreamer.cpp:128-236 (MelStreamer::makeTransposedBuffer / makeBuffer: one window of a streamed clip)
  *   wsp_set_mel               Whisper/source/whisper.h:107 whisper_set_mel
  *   wsp_encode                Whisper/source/whisper.h:117 whisper_encode          (Whisper/Whisper/WhisperContext.cpp:310 encode)
+ *   wsp_set_audio_ctx         Whisper/API/sFullParams.h:75 sFullParams::audio_ctx  (whisper_context::exp_n_audio_ctx, Whisper/source/whisper.cpp:2836)
  *   wsp_decode                Whisper/source/whisper.h:128 whisper_decode + :140-150 whisper_sample_best/timestamp
  *                             (Whisper/Whisper/WhisperContext.cpp:578 decode, Whisper/Whisper/ContextImpl.cpp:71-157 sampleBest)
  *   wsp_get_logits/probs      Whisper/source/whisper.h:166 whisper_get_probs
@@ -120,8 +121,19 @@ wsp_status wsp_set_mel( wsp_context* c, int32_t slot, const float* mel, int32_t 
 int32_t wsp_mel_len( wsp_context* c, int32_t slot );
 wsp_status wsp_get_mel( wsp_context* c, int32_t slot, float* dst, size_t cap_floats );
 
-/* a2-a12: encoder + cross-KV for slots [0,batch); mel_offsets[b] = first frame of the 3000-frame window (NULL = 0) */
+/* a2-a12: encoder + cross-KV for slots [0,batch); mel_offsets[b] = first frame of the 2n-frame window (NULL = 0), n = the audio context below */
 wsp_status wsp_encode( wsp_context* c, const int32_t* mel_offsets, int32_t batch );
+
+/* sFullParams::audio_ctx (Whisper/API/sFullParams.h:75): encode only the first n of the model's n_audio_ctx (1500) audio positions.
+ * As in the reference (whisper.cpp:1092-1167, 1479-1480, 1528; Whisper/Whisper/ContextImpl.cpp:24, 55, 489), the encoder then reads mel
+ * frames [offset, offset + 2n) — zero past the clip's end — convolves them with zero padding at frame 2n, adds the first n rows of the
+ * positional embedding and attends over n keys; the cross-K/V memories hold n rows per layer and every decoder cross-attention runs
+ * over those n keys.  Encoder work and cross-KV traffic fall in proportion to n.
+ * n <= 0 selects the default (n_audio_ctx); n > n_audio_ctx is WSP_E_INVALIDARG (the reference does not check it and would read past
+ * its positional table).  The value is context state and takes effect at the next wsp_encode, wsp_run_chunks* or wsp_detect_language;
+ * every decode attends over the n of the last encode, so the cross-KV layout and the decoder always agree.  wsp_get_tensor shapes
+ * follow that encode: "enc.input" [2n][80], "enc.conv1" [2n][d], "enc.x" / "encode-out" [n][d], "cross_k" / "cross_v" [L][H][n][64]. */
+wsp_status wsp_set_audio_ctx( wsp_context* c, int32_t n );
 
 /* a13-a18: one decoder call for `batch` chunks, n_tokens new tokens each (tokens[b*n_tokens + i]), after n_past cached ones.
  * sampled (nullable) receives the greedy choice per chunk from the last token's distribution. */
@@ -175,8 +187,9 @@ wsp_status wsp_timer_stop( wsp_context* c, float* ms );
  * around every launch.  kinds: 0 skinny GEMM, 1 cross-attention, 2 self-attention, 3 other (embedding, sampler) */
 wsp_status wsp_profile_decode( wsp_context* c, int32_t batch, int32_t n_steps, float ms_by_kind[ 4 ], int32_t launches_by_kind[ 4 ] );
 
-/* test hook: named intermediates as f32.  Names: "mel", "enc.conv1" ([3000][d] after GELU), "enc.x0" ([1500][d] input of layer 0),
- * "enc.layers" (residual stream after the last layer), "encode-out" (ln_post, f16-rounded), "cross_k", "cross_v" ([L][T][d] of slot 0). */
+/* test hook: named intermediates as f32.  Names: "mel", "enc.conv1" ([2n][d] after GELU), "enc.x0" ([n][d] input of layer 0),
+ * "enc.layers" (residual stream after the last layer), "encode-out" (ln_post, f16-rounded), "cross_k", "cross_v" ([L][T][d] of slot 0);
+ * n = the audio positions of the last encode (1500 unless wsp_set_audio_ctx chose fewer). */
 wsp_status wsp_get_tensor( wsp_context* c, const char* name, int32_t slot, float* dst, size_t cap_floats, size_t* n_floats );
 /* debug: run only the first n encoder layers (negative = all) */
 wsp_status wsp_debug_set_encoder_layers( wsp_context* c, int32_t n );

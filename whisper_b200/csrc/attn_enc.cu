@@ -1,4 +1,4 @@
-// Fused flash attention for the Whisper encoder on sm_90a (non-causal, head dim 64, T = 1500).
+// Fused flash attention for the Whisper encoder on sm_90a (non-causal, head dim 64, T = audio_ctx: 1500 unless overridden).
 //
 // Replaces flashAttention.hlsl / the mulMatTiled -> softMax -> mulMatTiled chain the reference actually runs
 // (Whisper/ML/Context.ops.cpp:194-227) and the CPU oracle's ggml_compute_forward_flash_attn_f16 (Whisper/source/ggml.c:5912-6097):

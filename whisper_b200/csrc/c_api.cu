@@ -284,7 +284,9 @@ wsp_status wsp_get_tensor( wsp_context* cc, const char* name, int32_t slot, floa
 	Context& c = *cc->c;
 	if( slot < 0 || slot >= c.maxB ) return fail( WSP_E_BOUNDS, "slot" );
 	const HParams& hp = c.e->hp;
-	const int d = hp.n_audio_state, T = hp.n_audio_ctx, L = hp.n_text_layer, H = hp.n_audio_head;
+	// shapes follow the last encode: T = its audio positions, 2T mel frames per chunk packed as 2T + 2 rows
+	const int d = hp.n_audio_state, T = c.encCtx, L = hp.n_text_layer, H = hp.n_audio_head;
+	const size_t rowsPad = (size_t)2 * T + 2;
 	WSP_CUDA( cudaSetDevice( c.e->device ) );
 	WSP_CUDA( cudaStreamSynchronize( c.stream ) );
 	const std::string nm( name );
@@ -292,9 +294,9 @@ wsp_status wsp_get_tensor( wsp_context* cc, const char* name, int32_t slot, floa
 	const __half* f16 = nullptr;
 	size_t n = 0;
 	if( nm == "mel" ) { f32 = c.slots[ slot ].mel; n = (size_t)80 * c.slots[ slot ].nLen; }
-	else if( nm == "enc.input" ) { f16 = c.melF16 + ( (size_t)slot * kFramesPad + 1 ) * 80; n = (size_t)kFrames * 80; }       // [3000][80]
-	else if( nm == "enc.conv1" ) { f16 = c.conv1 + ( (size_t)slot * kFramesPad + 1 ) * d; n = (size_t)kFrames * d; }           // [3000][d]
-	else if( nm == "enc.x" ) { f32 = c.x + (size_t)slot * T * d; n = (size_t)T * d; }                                             // [1500][d]
+	else if( nm == "enc.input" ) { f16 = c.melF16 + ( (size_t)slot * rowsPad + 1 ) * 80; n = (size_t)2 * T * 80; }             // [2T][80]
+	else if( nm == "enc.conv1" ) { f16 = c.conv1 + ( (size_t)slot * rowsPad + 1 ) * d; n = (size_t)2 * T * d; }                 // [2T][d]
+	else if( nm == "enc.x" ) { f32 = c.x + (size_t)slot * T * d; n = (size_t)T * d; }                                             // [T][d]
 	else if( nm == "enc.xn" || nm == "encode-out" ) { f16 = c.xn + (size_t)slot * T * d; n = (size_t)T * d; }
 	else if( nm == "enc.attn" ) { f16 = c.attn + (size_t)slot * T * d; n = (size_t)T * d; }
 	else if( nm == "enc.q" ) { f16 = c.q + (size_t)slot * T * d; n = (size_t)T * d; }                                             // [H][T][64]
@@ -312,7 +314,7 @@ wsp_status wsp_get_tensor( wsp_context* cc, const char* name, int32_t slot, floa
 		const __half* base = nm == "cross_k" ? c.crossK : c.crossV;
 		for( int l = 0; l < L; l++ )
 		{
-			const __half* src = base + ( (size_t)l * c.maxB + slot ) * T * d;
+			const __half* src = base + (size_t)l * c.maxB * hp.n_audio_ctx * d + (size_t)slot * T * d;
 			half_to_float_kernel<<<(unsigned)( ( (size_t)T * d + 255 ) / 256 ), 256>>>( src, tmp.p, (size_t)T * d );
 			WSP_CUDA( cudaMemcpy( dst + (size_t)l * T * d, tmp.p, (size_t)T * d * 4, cudaMemcpyDeviceToHost ) );
 		}
@@ -360,6 +362,11 @@ wsp_status wsp_detect_language( wsp_context* c, int32_t offset_frames, int32_t n
 		*lang_id = pid[ 0 ].second;
 		return WSP_OK;
 	} );
+}
+wsp_status wsp_set_audio_ctx( wsp_context* c, int32_t n )
+{
+	if( !c ) return fail( WSP_E_POINTER, "context" );
+	return ctxSetAudioCtx( *c->c, n );
 }
 wsp_status wsp_debug_set_encoder_layers( wsp_context* c, int32_t n )
 {

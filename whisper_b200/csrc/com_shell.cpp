@@ -934,11 +934,13 @@ namespace
 			logMessage( eLogLevel::Error, "whisper_b200: the SpeedupAudio flag is not implemented (nor is it by the reference's GPU model)" );
 			return E_NOTIMPL;
 		}
+		// audio_ctx <= 0 selects the model's n_audio_ctx, as in the reference; above it the reference would read past its positional
+		// embedding and cross-KV memories (whisper.cpp:1160-1167, 1479-1480), so it is refused here
 		const int nAudioCtx = eng->hp[ 1 ];
-		if( params.audio_ctx != 0 && params.audio_ctx != nAudioCtx )
+		if( params.audio_ctx > nAudioCtx )
 		{
-			logMessage( eLogLevel::Error, "whisper_b200: audio_ctx override is not supported" );
-			return E_NOTIMPL;
+			logMessage( eLogLevel::Error, "whisper_b200: audio_ctx %d exceeds the model's n_audio_ctx %d", params.audio_ctx, nAudioCtx );
+			return E_INVALIDARG;
 		}
 		// the reference's decoder arithmetic depends on its thread count (DESIGN.md §2); follow the caller's cpuThreads
 		const int threads = params.cpuThreads < 1 ? 1 : ( params.cpuThreads > 16 ? 16 : params.cpuThreads );
@@ -1123,6 +1125,9 @@ namespace
 		{
 			promptPast.insert( promptPast.begin(), params.prompt_tokens, params.prompt_tokens + params.prompt_n_tokens );
 		}
+		// audio_ctx is context state that whisper_full overwrites only here (:2836): AFTER language auto-detection, which therefore
+		// still encodes with the previous call's value, and not at all when the clip is shorter than 1 s (the return above)
+		HR( check( wsp_set_audio_ctx( ctx, params.audio_ctx ), "wsp_set_audio_ctx" ) );
 
 		std::vector<int32_t> promptInit = { tokSot };                                              // :2839-2848
 		if( multilingual )

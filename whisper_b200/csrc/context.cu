@@ -57,19 +57,21 @@ namespace wsp
 		const int d = hp.n_audio_state, H = hp.n_audio_head, T = hp.n_audio_ctx, L = hp.n_text_layer;
 		if( T * 2 != kFrames ) return fail( WSP_E_FORMAT, "n_audio_ctx must be 1500" );
 		c.Tp = ( ( T + 127 ) / 128 ) * 128;
+		c.encCtx = T;
 		WSP_CUDA( cudaStreamCreateWithFlags( &c.stream, cudaStreamNonBlocking ) );
 		for( auto& v : c.ev ) WSP_CUDA( cudaEventCreate( &v ) );
 		for( auto& v : c.timerEv ) WSP_CUDA( cudaEventCreate( &v ) );
 		c.slots.resize( maxBatch );
 		const size_t B = (size_t)maxBatch;
 		WSP_CHECK( devAlloc( c.melMax, B ) );
-		WSP_CHECK( devAlloc( c.melF16, B * kFramesPad * 80, true ) );          // halo rows stay zero forever
+		// the halo rows are rewritten by every encode (mel_window_kernel, EPI_CONV1) except row 0, which no packing moves
+		WSP_CHECK( devAlloc( c.melF16, B * kFramesPad * 80, true ) );
 		WSP_CHECK( devAlloc( c.conv1, B * kFramesPad * d, true ) );
 		WSP_CHECK( devAlloc( c.x, B * T * d ) );
 		WSP_CHECK( devAlloc( c.xn, B * T * d ) );
 		WSP_CHECK( devAlloc( c.q, B * T * d ) );
 		WSP_CHECK( devAlloc( c.k, B * T * d ) );
-		WSP_CHECK( devAlloc( c.vt, B * H * 64 * c.Tp, true ) );                // pad columns [T, Tp) stay zero
+		WSP_CHECK( devAlloc( c.vt, B * H * 64 * c.Tp, true ) );                // pad columns are re-zeroed by the QKV epilogue
 		WSP_CHECK( devAlloc( c.attn, B * T * d ) );
 		WSP_CHECK( devAlloc( c.h, B * T * 4 * d ) );
 		WSP_CHECK( devAlloc( c.crossK, (size_t)L * B * T * d ) );
@@ -317,7 +319,11 @@ namespace wsp
 	{
 		Engine& e = *c.e;
 		const HParams& hp = e.hp;
-		const int d = hp.n_audio_state, H = hp.n_audio_head, T = hp.n_audio_ctx, L = hp.n_text_layer;
+		const int d = hp.n_audio_state, H = hp.n_audio_head, L = hp.n_text_layer;
+		// audio positions of this encode (whisper.cpp:1092): the window is 2T mel frames, every chunk takes 2T + 2 rows (halo, frames,
+		// halo) in melF16 / conv1 and T rows everywhere after conv2
+		const int T = c.audioCtx > 0 ? c.audioCtx : hp.n_audio_ctx;
+		const int frames = 2 * T, rowsPad = frames + 2;
 		cudaStream_t s = c.stream;
 		for( int b = 0; b < batch; b++ )
 		{
@@ -325,23 +331,25 @@ namespace wsp
 			if( !ms.mel ) return fail( WSP_E_INVALIDARG, "no mel in slot " + std::to_string( b ) );
 			const int off = offsets ? offsets[ b ] : 0;
 			if( off < 0 ) return fail( WSP_E_INVALIDARG, "negative mel offset" );
-			WSP_CUDA( kern::melWindow( ms.mel, ms.nLen, off, c.melF16 + (size_t)b * kFramesPad * 80, kFrames, s ) );
+			WSP_CUDA( kern::melWindow( ms.mel, ms.nLen, off, c.melF16 + (size_t)b * rowsPad * 80, frames, s ) );
 			launched();
 		}
+		// from here on the cross-KV memories are (being) rewritten with T rows per chunk: decodes attend over T keys
+		c.encCtx = T;
 		gemm::Launch g;
 		// conv1 + bias + GELU -> f16, time-major with halo (a3)
 		g = gemm::Launch();
 		g.mapA = c.mapMel; g.mapA2 = c.mapMel; g.mapB = c.mapConv1W;
-		g.M = batch * kFramesPad - 2; g.N = d; g.K = 3 * kConv1KTap; g.kTap = kConv1KTap / gemm::BK;
+		g.M = batch * rowsPad - 2; g.N = d; g.K = 3 * kConv1KTap; g.kTap = kConv1KTap / gemm::BK;
 		g.ep.M = g.M; g.ep.N = d; g.ep.ld = d; g.ep.bias = e.conv1b; g.ep.out_a = c.conv1;
-		g.ep.rows_per_chunk = kFramesPad; g.ep.valid_per_chunk = kFrames; g.ep.nchunks = batch;
+		g.ep.rows_per_chunk = rowsPad; g.ep.valid_per_chunk = frames; g.ep.nchunks = batch;
 		WSP_CUDA( gemm::launch( g, gemm::EPI_CONV1, gemm::A_CONV_S1, c.bnD, e.numSMs, s ) );
 		// conv2 (stride 2) + bias + GELU + positional embedding -> f32 residual stream (a4)
 		g = gemm::Launch();
 		g.mapA = c.mapConv1Even; g.mapA2 = c.mapConv1Odd; g.mapB = c.mapConv2W;
-		g.M = batch * ( kFramesPad / 2 ) - 1; g.N = d; g.K = 3 * d; g.kTap = d / gemm::BK;
+		g.M = batch * ( rowsPad / 2 ) - 1; g.N = d; g.K = 3 * d; g.kTap = d / gemm::BK;
 		g.ep.M = g.M; g.ep.N = d; g.ep.ld = d; g.ep.bias = e.conv2b; g.ep.pos = e.encPos; g.ep.out_f32 = c.x;
-		g.ep.rows_per_chunk = kFramesPad / 2; g.ep.valid_per_chunk = T; g.ep.nchunks = batch; g.ep.T = T; g.ep.d = d;
+		g.ep.rows_per_chunk = rowsPad / 2; g.ep.valid_per_chunk = T; g.ep.nchunks = batch; g.ep.T = T; g.ep.d = d;
 		WSP_CUDA( gemm::launch( g, gemm::EPI_CONV2, gemm::A_CONV_S2, c.bnD, e.numSMs, s ) );
 		launched( 2 );
 
@@ -390,9 +398,18 @@ namespace wsp
 		g.M = M; g.N = L * 2 * d; g.K = d;
 		g.ep.M = M; g.ep.N = g.N; g.ep.bias = e.crossB; g.ep.out_a = c.crossK; g.ep.out_b = c.crossV;
 		g.ep.T = T; g.ep.H = H; g.ep.d = d; g.ep.nchunks = c.maxB;
+		g.ep.layer_stride = (size_t)c.maxB * hp.n_audio_ctx * d;   // [L][maxB][H][T][64] inside the 1500-row layers of the pointer tables
 		g.ep.scale = (float)pow( 64.0, -0.25 );   // whisper.cpp:1465
 		WSP_CUDA( gemm::launch( g, gemm::EPI_CROSSKV, gemm::A_PLAIN, c.bnCross, e.numSMs, s ) );
 		launched( 2 );
+		return WSP_OK;
+	}
+
+	// whisper_full's audio_ctx (whisper.cpp:1092, 1528, 2836): encode only the first n audio positions; n <= 0 = the model's own
+	int ctxSetAudioCtx( Context& c, int n )
+	{
+		if( n > c.e->hp.n_audio_ctx ) return fail( WSP_E_INVALIDARG, "audio_ctx exceeds the model's n_audio_ctx" );
+		c.audioCtx = n > 0 ? n : 0;
 		return WSP_OK;
 	}
 
@@ -446,7 +463,8 @@ namespace wsp
 	{
 		Engine& e = *c.e;
 		const HParams& hp = e.hp;
-		const int d = hp.n_text_state, H = hp.n_text_head, T = hp.n_audio_ctx, nCtx = hp.n_text_ctx;
+		// T = cross-attention keys: the audio positions of the last encode (whisper.cpp:1528)
+		const int d = hp.n_text_state, H = hp.n_text_head, T = c.encCtx, nCtx = hp.n_text_ctx;
 		cudaStream_t s = c.stream;
 		const int cols = batch * N;
 		const float qkScale = (float)pow( 64.0, -0.25 );   // whisper.cpp:1588, 1595, 1700
@@ -520,7 +538,7 @@ namespace wsp
 			a.W = W.wcq; a.nOut = d; a.K = d; a.xF32 = c.xd; a.xStride = d; a.gamma = W.lnc.g; a.beta = W.lnc.b; a.nCols = cols;
 			a.epi = kern::SK_Q_SCALE; a.bias = W.bcq; a.scale = qkScale; a.outF32 = c.qd; a.ld = d;
 			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( a, s ) );
-			const size_t crossOff = (size_t)il * c.maxB * T * d;
+			const size_t crossOff = (size_t)il * c.maxB * hp.n_audio_ctx * d;   // layer stride of the pointer tables, whatever T is
 			WSP_KERNEL( KK_CROSS, kern::crossAttnDecode( c.qd, c.crossK + crossOff, c.crossV + crossOff, c.attnD, batch, N, H, d, T, c.refThreads, s ) );
 			a = kern::SkinnyArgs();
 			a.W = W.wco; a.nOut = d; a.K = d; a.xF16 = c.attnD; a.xStride = d; a.nCols = cols;
@@ -565,7 +583,7 @@ namespace wsp
 		int n = 0;
 		if( N == 1 && !allLogits && sample && c.useGraph && !c.prof.on )
 		{
-			if( !c.stepGraph || c.stepGraphBatch != batch )
+			if( !c.stepGraph || c.stepGraphBatch != batch || c.stepGraphCtx != c.encCtx )
 			{
 				if( c.stepGraph ) { cudaGraphExecDestroy( c.stepGraph ); c.stepGraph = nullptr; }
 				cudaGraph_t graph = nullptr;
@@ -578,6 +596,7 @@ namespace wsp
 				cudaGraphDestroy( graph );
 				WSP_CUDA( ce );
 				c.stepGraphBatch = batch;
+				c.stepGraphCtx = c.encCtx;
 				c.stepGraphLaunches = n;
 			}
 			WSP_CUDA( cudaGraphLaunch( c.stepGraph, c.stream ) );

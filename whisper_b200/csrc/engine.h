@@ -116,18 +116,22 @@ namespace wsp
 		uint64_t devBytes = 0;          // device memory this context holds (timingsPrint's memory table)
 
 		// encoder workspaces
+		// sized for n_audio_ctx = 1500; an encode over n <= 1500 audio positions (audio_ctx) packs its chunks densely with n in
+		// place of 1500 (2n + 2 rows per chunk in melF16 / conv1), inside the same allocations and tensor maps
 		__half* melF16 = nullptr;       // [maxB][3002][80]
 		__half* conv1 = nullptr;        // [maxB][3002][d]
 		float* x = nullptr;             // [maxB*1500][d] residual stream
 		__half* xn = nullptr;           // [maxB*1500][d]
 		__half* q = nullptr;            // [maxB][H][1500][64]
 		__half* k = nullptr;
-		__half* vt = nullptr;           // [maxB][H][64][Tp]
+		__half* vt = nullptr;           // [maxB][H][64][Tp] (row length Tp whatever n is)
 		__half* attn = nullptr;         // [maxB*1500][d]
 		__half* h = nullptr;            // [maxB*1500][4d]
-		__half* crossK = nullptr;       // [L][maxB][H][1500][64]
+		__half* crossK = nullptr;       // [L][maxB][H][1500][64]; with n audio positions each layer holds [maxB][H][n][64] at the same stride
 		__half* crossV = nullptr;
 		int Tp = 0;
+		int audioCtx = 0;               // audio positions the next encode uses (wsp_set_audio_ctx; 0 = the model's n_audio_ctx)
+		int encCtx = 0;                 // audio positions of the last encode: rows of the cross-KV memories every decode attends over
 
 		// decoder state
 		__half* selfK = nullptr;        // [L][maxB][H][n_text_ctx][64] (head-major rows)
@@ -176,6 +180,7 @@ namespace wsp
 		// decode CUDA graph (N = 1 steady state)
 		cudaGraphExec_t stepGraph = nullptr;
 		int stepGraphBatch = 0;
+		int stepGraphCtx = 0;           // encCtx the graph was captured for (the step kernels take it by value)
 		int stepGraphLaunches = 0;
 		bool useGraph = true;
 
@@ -195,6 +200,7 @@ namespace wsp
 	int ctxPcmToMelWindow( Context& c, int slot, const float* pcmHost, int nSamples, int nFrames, const float* forcedMax, float* maxOut );
 	int ctxSetMel( Context& c, int slot, const float* melHost, int nLen );
 	int ctxEncode( Context& c, const int32_t* offsets, int batch );
+	int ctxSetAudioCtx( Context& c, int n );
 	int ctxDecode( Context& c, const int32_t* tokensHost, int nTokens, int nPast, int batch, uint32_t flags, wsp_token_data* sampledHost );
 	int ctxUploadPcm( Context& c, int slot, const float* pcmHost, int nSamples );
 	int ctxProfileDecode( Context& c, int batch, int nSteps, float* msByKind, int* launchesByKind );

@@ -61,7 +61,19 @@ namespace gemm
 		{
 			const int b = m / ep.rows_per_chunk;
 			const int t = m - b * ep.rows_per_chunk;
-			if( b >= ep.nchunks || t >= ep.valid_per_chunk ) return;
+			if( b >= ep.nchunks ) return;
+			if( t >= ep.valid_per_chunk )
+			{
+				// the two rows past a chunk's frames are its trailing halo and the next chunk's leading one (conv2's zero padding):
+				// rewritten on every call, because where they lie depends on audio_ctx (row 0, the first chunk's halo, never moves)
+				if( m + 1 < ep.nchunks * ep.rows_per_chunk )
+				{
+#pragma unroll
+					for( int i = 0; i < 32; i++ ) v[ i ] = 0.0f;
+					store_f16x32( ep.out_a + (size_t)( m + 1 ) * ep.ld + n0, v );
+				}
+				return;
+			}
 #pragma unroll
 			for( int i = 0; i < 32; i++ )
 				v[ i ] = ptx::gelu_f16_semantics( v[ i ] + ep.bias[ n0 + i ] );
@@ -109,6 +121,15 @@ namespace gemm
 #pragma unroll
 				for( int i = 0; i < 32; i++ )
 					dst[ (size_t)i * ep.Tp ] = __float2half_rn( v[ i ] );
+				// V^T columns [T, T rounded up to 128) are read by the attention's last key tile: masked keys get P = 0, but 0 times a
+				// stale Inf from an earlier, longer audio_ctx would be NaN.  Time step t clears columns T + t, T + t + T, ...
+				const int tEnd = ( ep.T + 127 ) & ~127;
+				for( int tz = ep.T + t; tz < tEnd; tz += ep.T )
+				{
+#pragma unroll
+					for( int i = 0; i < 32; i++ )
+						dst[ (size_t)i * ep.Tp + ( tz - t ) ] = __float2half_rn( 0.0f );
+				}
 			}
 		}
 		else if constexpr( MODE == EPI_BIAS_RESID )
@@ -160,8 +181,8 @@ namespace gemm
 				for( int i = 0; i < 32; i++ )
 					v[ i ] *= ep.scale;
 			}
-			__half* base = isV ? ep.out_b : ep.out_a;
-			store_f16x32( base + ( ( ( (size_t)l * ep.nchunks + b ) * ep.H + h ) * ep.T + t ) * 64 + e, v );
+			__half* base = ( isV ? ep.out_b : ep.out_a ) + (size_t)l * ep.layer_stride;
+			store_f16x32( base + ( ( (size_t)b * ep.H + h ) * ep.T + t ) * 64 + e, v );
 		}
 	}
 
@@ -197,6 +218,8 @@ namespace gemm
 			{
 				if( cb < ep.nchunks && t < ep.valid_per_chunk )
 					ep.out_a[ (size_t)( mBase + rr + 1 ) * ep.ld + n ] = __float2half_rn( ptx::gelu_f16_semantics( w[ rr * STG_LD ] + b ) );
+				else if( cb < ep.nchunks && mBase + rr + 1 < ep.nchunks * ep.rows_per_chunk )
+					ep.out_a[ (size_t)( mBase + rr + 1 ) * ep.ld + n ] = __float2half_rn( 0.0f );   // halo rows, as in epilogue<EPI_CONV1>
 				if( ++t == ep.rows_per_chunk ) { t = 0; cb++; }
 			}
 		}
@@ -291,14 +314,14 @@ namespace gemm
 			const int h = nn >> 6, e = nn & 63;
 			const float b = isV ? ep.bias[ n ] : 0.0f;
 			const float sc = isV ? 1.0f : ep.scale;
-			__half* base = isV ? ep.out_b : ep.out_a;
+			__half* base = ( isV ? ep.out_b : ep.out_a ) + (size_t)l * ep.layer_stride;
 			int cb = mBase / ep.T;
 			int t = mBase - cb * ep.T;
 #pragma unroll
 			for( int rr = 0; rr < 32; rr++ )
 			{
 				if( mBase + rr < ep.M )
-					base[ ( ( ( (size_t)l * ep.nchunks + cb ) * ep.H + h ) * ep.T + t ) * 64 + e ] = __float2half_rn( w[ rr * STG_LD ] * sc + b );
+					base[ ( ( (size_t)cb * ep.H + h ) * ep.T + t ) * 64 + e ] = __float2half_rn( w[ rr * STG_LD ] * sc + b );
 				if( ++t == ep.T ) { t = 0; cb++; }
 			}
 		}

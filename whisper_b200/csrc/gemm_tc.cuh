@@ -25,7 +25,7 @@ namespace gemm
 	enum EpiMode : int
 	{
 		EPI_F32 = 0,          // out_f32[m][n] = acc (+ bias[n])                                  (tests, decoder prompt)
-		EPI_CONV1 = 1,        // f16 out[(m+1)][n] = gelu(acc + bias[n]), rows of padded time axis  (a3)
+		EPI_CONV1 = 1,        // f16 out[(m+1)][n] = gelu(acc + bias[n]), rows of padded time axis, halos zeroed (a3)
 		EPI_CONV2 = 2,        // f32 out[b*T+j][n] = gelu(acc + bias[n]) + pos[j][n]                (a4)
 		EPI_QKV = 3,          // Q,K head-major f16, V transposed f16                               (a6, a7)
 		EPI_BIAS_RESID = 4,   // f32 out[m][n] = acc + bias[n] + resid[m][n]                        (a9, a10)
@@ -53,13 +53,14 @@ namespace gemm
 		__half* out_a = nullptr;   // Q | conv1 out | gelu out | cross K
 		__half* out_b = nullptr;   // K | cross V
 		__half* out_c = nullptr;   // V^T
-		int T = 0;                 // time steps per chunk (1500)
+		int T = 0;                 // time steps per chunk (audio_ctx, 1500 by default)
 		int Tp = 0;                // padded row length of V^T
 		int H = 0;                 // heads
 		int d = 0;                 // model width
 		int rows_per_chunk = 0;    // conv: padded rows per chunk in the flattened A row space
 		int valid_per_chunk = 0;   // conv: valid output rows per chunk
 		int nchunks = 0;
+		size_t layer_stride = 0;   // EPI_CROSSKV: elements between two decoder layers' memories
 		float scale = 1.0f;
 	};
 

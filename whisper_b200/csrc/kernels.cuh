@@ -52,7 +52,8 @@ namespace kern
 	cudaError_t melPower( const MelTables& tb, const float* pcm, int nSamples, int nLen, float* melRaw, int* maxSlot, cudaStream_t s );
 	// in place: clamp to (max - 8), (x + 4) / 4
 	cudaError_t melNormalize( float* mel, int count, const int* maxSlot, cudaStream_t s );
-	// mel f32 [80][nLen] at frame offset -> time-major f16 window [1 + 3000 + 1][80] with zero halo rows (conv padding)
+	// mel f32 [80][nLen] at frame offset -> time-major f16 window [1 + frames + 1][80], halo rows (conv padding) written as zeros;
+	// frames = 2 * audio_ctx (3000 by default)
 	cudaError_t melWindow( const float* mel, int nLen, int offset, __half* dst, int frames, cudaStream_t s );
 
 	// ---- LayerNorm + affine -> f16 (a5, a11) -------------------------------------------------------------------------

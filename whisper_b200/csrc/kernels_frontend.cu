@@ -189,31 +189,33 @@ namespace kern
 
 	// ---------------------------------------------------------------------------------------------------------------
 	// window gather: mel[80][nLen] (band-major) -> f16 [1 + frames + 1][80] (time-major) at `offset`, zero beyond nLen
-	// (whisper.cpp:1104-1120 copies the slice and zero-pads; the f16 rounding is ggml's conv input conversion, ggml.c:5275-5283)
+	// (whisper.cpp:1104-1120 copies the slice and zero-pads; the f16 rounding is ggml's conv input conversion, ggml.c:5275-5283).
+	// Row r holds frame r - 1; rows 0 and frames + 1 are conv1's zero padding and are written here too: where they lie depends on
+	// the window length (2 * audio_ctx frames), which may change from one encode to the next.
 	__global__ void __launch_bounds__( 256 )
 		mel_window_kernel( const float* __restrict__ mel, int nLen, int offset, __half* __restrict__ dst, int frames )
 	{
 		__shared__ float tile[ MEL_BANDS ][ 33 ];
-		const int t0 = blockIdx.x * 32;
+		const int r0 = blockIdx.x * 32;
 		for( int i = threadIdx.x; i < MEL_BANDS * 32; i += blockDim.x )
 		{
 			const int c = i >> 5, tt = i & 31;
-			const int t = t0 + tt;
+			const int t = r0 + tt - 1;
 			const int src = offset + t;
-			tile[ c ][ tt ] = ( t < frames && src < nLen ) ? mel[ (size_t)c * nLen + src ] : 0.0f;
+			tile[ c ][ tt ] = ( t >= 0 && t < frames && src < nLen ) ? mel[ (size_t)c * nLen + src ] : 0.0f;
 		}
 		__syncthreads();
 		for( int i = threadIdx.x; i < MEL_BANDS * 32; i += blockDim.x )
 		{
 			const int tt = i / MEL_BANDS, c = i - tt * MEL_BANDS;
-			const int t = t0 + tt;
-			if( t < frames )
-				dst[ (size_t)( t + 1 ) * MEL_BANDS + c ] = __float2half_rn( tile[ c ][ tt ] );
+			const int r = r0 + tt;
+			if( r < frames + 2 )
+				dst[ (size_t)r * MEL_BANDS + c ] = __float2half_rn( tile[ c ][ tt ] );
 		}
 	}
 	cudaError_t melWindow( const float* mel, int nLen, int offset, __half* dst, int frames, cudaStream_t s )
 	{
-		mel_window_kernel<<<( frames + 31 ) / 32, 256, 0, s>>>( mel, nLen, offset, dst, frames );
+		mel_window_kernel<<<( frames + 2 + 31 ) / 32, 256, 0, s>>>( mel, nLen, offset, dst, frames );
 		return cudaGetLastError();
 	}
 
