@@ -386,7 +386,7 @@ wsp_status wsp_debug_step_timing( wsp_context* c, uint64_t* dst, int32_t cap )
 {
 	if( !c || !dst ) return fail( WSP_E_POINTER, "context/dst" );
 	WSP_CUDA( cudaStreamSynchronize( c->c->stream ) );
-	WSP_CUDA( cudaMemcpy( dst, c->c->megaTiming, sizeof( uint64_t ) * (size_t)( cap < 4608 ? cap : 4608 ), cudaMemcpyDeviceToHost ) );
+	WSP_CUDA( cudaMemcpy( dst, c->c->stepMarks, sizeof( uint64_t ) * (size_t)( cap < kStepMarks ? cap : kStepMarks ), cudaMemcpyDeviceToHost ) );
 	return WSP_OK;
 }
 wsp_status wsp_debug_set_step_mode( wsp_context* c, int32_t on )

@@ -36,7 +36,7 @@ namespace wsp
 		for( auto& s : slots ) { if( s.mel ) cudaFree( s.mel ); if( s.pcm ) cudaFree( s.pcm ); }
 		for( auto& v : prof.pool ) cudaEventDestroy( v );
 		for( auto& v : timerEv ) if( v ) cudaEventDestroy( v );
-		void* bufs[] = { flowLayers, flowBias, flowExch, flowCtrl, megaLayers, megaBarrier, megaTiming, melMax, pcmDev, melF16, conv1, x, xn, q, k, vt, attn, h, crossK, crossV, selfK, selfV, xd, qd, attnD, hD, logits, probs, tieScratch,
+		void* bufs[] = { flowLayers, flowBias, flowExch, flowCtrl, megaLayers, megaBarrier, stepMarks, melMax, pcmDev, melF16, conv1, x, xn, q, k, vt, attn, h, crossK, crossV, selfK, selfV, xd, qd, attnD, hD, logits, probs, tieScratch,
 			tokensDev, dNPast, sampled, history };
 		for( void* b : bufs ) if( b ) cudaFree( b );
 		for( auto& v : ev ) if( v ) cudaEventDestroy( v );
@@ -121,55 +121,44 @@ namespace wsp
 		ok &= gemm::makeMap2D( &c.mapK, c.k, 64, B * H * T, 128, 128 );
 		ok &= gemm::makeMap2D( &c.mapVt, c.vt, c.Tp, B * H * 64, (uint64_t)c.Tp * 2, 64 );
 		if( !ok ) return fail( WSP_E_CUDA, "cuTensorMapEncodeTiled failed (driver too old for TMA?)" );
-		// per-layer pointer table for the persistent decoder-step kernel
-		{
-			std::vector<kern::MegaLayer> ml( (size_t)L );
-			for( int i = 0; i < L; i++ )
-			{
-				const DecLayerW& W = e->dec[ i ];
-				kern::MegaLayer& m = ml[ i ];
-				m.ln1g = W.ln1.g; m.ln1b = W.ln1.b; m.lncg = W.lnc.g; m.lncb = W.lnc.b; m.ln3g = W.ln3.g; m.ln3b = W.ln3.b;
-				m.wqkv = W.wqkv; m.wo = W.wo; m.wcq = W.wcq; m.wco = W.wco; m.w1 = W.w1; m.w2 = W.w2;
-				m.bqkv = W.bqkv; m.bo = W.bo; m.bcq = W.bcq; m.bco = W.bco; m.b1 = W.b1; m.b2 = W.b2;
-				m.kCache = c.selfK + (size_t)i * B * hp.n_text_ctx * d;
-				m.vCache = c.selfV + (size_t)i * B * hp.n_text_ctx * d;
-				m.crossK = c.crossK + (size_t)i * B * T * d;
-				m.crossV = c.crossV + (size_t)i * B * T * d;
-			}
-			WSP_CHECK( devAlloc( c.megaLayers, (size_t)L ) );
-			WSP_CUDA( cudaMemcpy( c.megaLayers, ml.data(), ml.size() * sizeof( kern::MegaLayer ), cudaMemcpyHostToDevice ) );
-			WSP_CHECK( devAlloc( c.megaBarrier, 64, true ) );
-			WSP_CHECK( devAlloc( c.megaTiming, 4608, true ) );
-		}
-		// dataflow decoder-step kernel: pointer table, per-CTA bias slabs, sentinel-filled exchange buffers (decode_flow.cu)
+		// per-layer pointer tables of the two decoder-step kernels: the persistent one (decode_mega.cu) and the dataflow one
+		// (decode_flow.cu, which also gets per-CTA bias slabs and sentinel-filled exchange buffers)
 		{
 			const kern::FlowGeom g = kern::flowGeometry( d, hp.n_vocab, e->numSMs );
 			c.flowGeom = g;
 			const size_t slabLayer = (size_t)g.grid * g.slabFloats;
 			WSP_CHECK( devAlloc( c.flowBias, slabLayer * L ) );
+			std::vector<kern::MegaLayer> ml( (size_t)L );
 			std::vector<kern::FlowLayer> fl( (size_t)L );
 			for( int i = 0; i < L; i++ )
 			{
 				const DecLayerW& W = e->dec[ i ];
-				kern::FlowLayer& m = fl[ i ];
-				m.ln1g = W.ln1.g; m.ln1b = W.ln1.b; m.lncg = W.lnc.g; m.lncb = W.lnc.b; m.ln3g = W.ln3.g; m.ln3b = W.ln3.b;
-				m.wqkv = W.wqkv; m.wo = W.wo; m.wcq = W.wcq; m.wco = W.wco; m.w1 = W.w1; m.w2 = W.w2;
-				m.biasSlab = c.flowBias + (size_t)i * slabLayer;
-				m.kCache = c.selfK + (size_t)i * B * hp.n_text_ctx * d;
-				m.vCache = c.selfV + (size_t)i * B * hp.n_text_ctx * d;
-				m.crossK = c.crossK + (size_t)i * B * T * d;
-				m.crossV = c.crossV + (size_t)i * B * T * d;
+				auto common = [ & ]( auto& m ) {
+					m.ln1g = W.ln1.g; m.ln1b = W.ln1.b; m.lncg = W.lnc.g; m.lncb = W.lnc.b; m.ln3g = W.ln3.g; m.ln3b = W.ln3.b;
+					m.wqkv = W.wqkv; m.wo = W.wo; m.wcq = W.wcq; m.wco = W.wco; m.w1 = W.w1; m.w2 = W.w2;
+					m.kCache = c.selfK + (size_t)i * B * hp.n_text_ctx * d;
+					m.vCache = c.selfV + (size_t)i * B * hp.n_text_ctx * d;
+					m.crossK = c.crossK + (size_t)i * B * T * d;
+					m.crossV = c.crossV + (size_t)i * B * T * d;
+				};
+				kern::MegaLayer& m = ml[ i ];
+				common( m );
+				m.bqkv = W.bqkv; m.bo = W.bo; m.bcq = W.bcq; m.bco = W.bco; m.b1 = W.b1; m.b2 = W.b2;
+				common( fl[ i ] );
+				fl[ i ].biasSlab = c.flowBias + (size_t)i * slabLayer;
 				WSP_CUDA( kern::flowBuildBiasSlab( c.flowBias + (size_t)i * slabLayer, g, d, W.bqkv, W.bo, W.bcq, W.bco, W.b1, W.b2, c.stream ) );
 			}
+			WSP_CHECK( devAlloc( c.megaLayers, (size_t)L ) );
+			WSP_CUDA( cudaMemcpy( c.megaLayers, ml.data(), ml.size() * sizeof( kern::MegaLayer ), cudaMemcpyHostToDevice ) );
 			WSP_CHECK( devAlloc( c.flowLayers, (size_t)L ) );
 			WSP_CUDA( cudaMemcpy( c.flowLayers, fl.data(), fl.size() * sizeof( kern::FlowLayer ), cudaMemcpyHostToDevice ) );
+			WSP_CHECK( devAlloc( c.megaBarrier, 64, true ) );
 			const size_t exBytes = kern::flowExchangeBytes( d, maxBatch, L );
 			WSP_CHECK( devAlloc( c.flowExch, exBytes ) );
 			WSP_CUDA( cudaMemset( c.flowExch, 0xFF, exBytes ) );
 			WSP_CHECK( devAlloc( c.flowCtrl, 8, true ) );
-			const char* env = getenv( "WSP_STEP_MODE" );
-			if( env && env[ 0 ] >= '0' && env[ 0 ] <= '2' ) c.stepMode = env[ 0 ] - '0';
-			env = getenv( "WSP_TIMING_CTA" );
+			WSP_CHECK( devAlloc( c.stepMarks, kStepMarks, true ) );
+			const char* env = getenv( "WSP_TIMING_CTA" );
 			if( env ) c.stepTimingCta = atoi( env );
 		}
 		WSP_CUDA( kern::prepare( 4 * d ) );
@@ -457,6 +446,20 @@ namespace wsp
 	}
 #define WSP_KERNEL( kind, expr ) do { ProfScope _ps( c, kind ); WSP_CUDA( expr ); } while( 0 )
 
+	// Greedy sampling of the last token of every chunk from c.logits (sampler + advance kernel): the next tokens, n_past and the
+	// step counter stay on the device
+	static int enqueueSampler( Context& c, int N, int batch )
+	{
+		const Engine& e = *c.e;
+		kern::SampleArgs sa;
+		sa.logits = c.logits; sa.probs = c.probs; sa.tieScratch = c.tieScratch; sa.B = batch; sa.nVocab = e.hp.n_vocab;
+		sa.tokenBeg = e.tokBeg; sa.tokenSot = e.tokSot; sa.tokenSolm = e.tokSolm; sa.tokenNot = e.tokNot;
+		sa.dForceTs = c.dFlags; sa.out = c.sampled; sa.nextTokens = c.tokensDev; sa.dNPast = c.dNPast; sa.N = N;
+		sa.history = c.history; sa.histCap = c.histCap; sa.dStep = c.dStep;
+		WSP_KERNEL( KK_OTHER, kern::sampleGreedy( sa, c.stream ) );
+		return WSP_OK;
+	}
+
 	// Enqueue one decoder pass for `batch` chunks x N tokens.  Reads tokens from c.tokensDev, n_past / sampling flags from device
 	// scalars (so the N = 1 instance can be captured once as a CUDA graph and replayed for every step).
 	static int decodeEnqueue( Context& c, int N, int batch, bool allLogits, bool sample, int* launchesOut )
@@ -477,19 +480,11 @@ namespace wsp
 			fa.refThreads = c.refThreads;
 			fa.tokEmb = e.tokEmb; fa.decPos = e.decPos; fa.lnfg = e.decLn.g; fa.lnfb = e.decLn.b;
 			fa.tokens = c.tokensDev; fa.dNPast = c.dNPast;
-			fa.exch = c.flowExch; fa.ctrl = c.flowCtrl; fa.logits = c.logits; fa.timing = c.stepTiming ? c.megaTiming : nullptr;
+			fa.exch = c.flowExch; fa.ctrl = c.flowCtrl; fa.logits = c.logits; fa.timing = c.stepTiming ? c.stepMarks : nullptr;
 			fa.g = c.flowGeom;
 			fa.timingCta = c.stepTimingCta;
 			WSP_KERNEL( KK_SKINNY, kern::decodeStepFlow( fa, d, e.numSMs, s ) ); n++;
-			if( sample )
-			{
-				kern::SampleArgs sa;
-				sa.logits = c.logits; sa.probs = c.probs; sa.tieScratch = c.tieScratch; sa.B = batch; sa.nVocab = hp.n_vocab;
-				sa.tokenBeg = e.tokBeg; sa.tokenSot = e.tokSot; sa.tokenSolm = e.tokSolm; sa.tokenNot = e.tokNot;
-				sa.dForceTs = c.dFlags; sa.out = c.sampled; sa.nextTokens = c.tokensDev; sa.dNPast = c.dNPast; sa.N = N;
-				sa.history = c.history; sa.histCap = c.histCap; sa.dStep = c.dStep;
-				WSP_KERNEL( KK_OTHER, kern::sampleGreedy( sa, s ) ); n += 2;
-			}
+			if( sample ) { WSP_CHECK( enqueueSampler( c, N, batch ) ); n += 2; }
 			if( launchesOut ) *launchesOut = n;
 			return WSP_OK;
 		}
@@ -501,17 +496,9 @@ namespace wsp
 			ma.refThreads = c.refThreads;
 			ma.tokEmb = e.tokEmb; ma.decPos = e.decPos; ma.lnfg = e.decLn.g; ma.lnfb = e.decLn.b;
 			ma.tokens = c.tokensDev; ma.dNPast = c.dNPast;
-			ma.x = c.xd; ma.q = c.qd; ma.attn = c.attnD; ma.h = c.hD; ma.logits = c.logits; ma.barrier = c.megaBarrier; ma.timing = c.stepTiming ? c.megaTiming : nullptr;
+			ma.x = c.xd; ma.q = c.qd; ma.attn = c.attnD; ma.h = c.hD; ma.logits = c.logits; ma.barrier = c.megaBarrier; ma.timing = c.stepTiming ? c.stepMarks : nullptr;
 			WSP_KERNEL( KK_SKINNY, kern::decodeStepMega( ma, d, e.numSMs, s ) ); n++;
-			if( sample )
-			{
-				kern::SampleArgs sa;
-				sa.logits = c.logits; sa.probs = c.probs; sa.tieScratch = c.tieScratch; sa.B = batch; sa.nVocab = hp.n_vocab;
-				sa.tokenBeg = e.tokBeg; sa.tokenSot = e.tokSot; sa.tokenSolm = e.tokSolm; sa.tokenNot = e.tokNot;
-				sa.dForceTs = c.dFlags; sa.out = c.sampled; sa.nextTokens = c.tokensDev; sa.dNPast = c.dNPast; sa.N = N;
-				sa.history = c.history; sa.histCap = c.histCap; sa.dStep = c.dStep;
-				WSP_KERNEL( KK_OTHER, kern::sampleGreedy( sa, s ) ); n += 2;
-			}
+			if( sample ) { WSP_CHECK( enqueueSampler( c, N, batch ) ); n += 2; }
 			if( launchesOut ) *launchesOut = n;
 			return WSP_OK;
 		}
@@ -564,15 +551,7 @@ namespace wsp
 			a.epi = kern::SK_LOGITS; a.outF32 = c.logits; a.ld = hp.n_vocab;
 			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( a, s ) ); n++;
 		}
-		if( sample && !allLogits )
-		{
-			kern::SampleArgs sa;
-			sa.logits = c.logits; sa.probs = c.probs; sa.tieScratch = c.tieScratch; sa.B = batch; sa.nVocab = hp.n_vocab;
-			sa.tokenBeg = e.tokBeg; sa.tokenSot = e.tokSot; sa.tokenSolm = e.tokSolm; sa.tokenNot = e.tokNot;
-			sa.dForceTs = c.dFlags; sa.out = c.sampled; sa.nextTokens = c.tokensDev; sa.dNPast = c.dNPast; sa.N = N;
-			sa.history = c.history; sa.histCap = c.histCap; sa.dStep = c.dStep;
-			WSP_KERNEL( KK_OTHER, kern::sampleGreedy( sa, s ) ); n += 2;
-		}
+		if( sample && !allLogits ) { WSP_CHECK( enqueueSampler( c, N, batch ) ); n += 2; }
 		if( launchesOut ) *launchesOut = n;
 		return WSP_OK;
 	}

@@ -76,25 +76,6 @@ namespace kern
 		}
 
 		// ---- small device helpers ------------------------------------------------------------------------------------
-		__device__ __forceinline__ float warpSumF( float v )
-		{
-			for( int o = 16; o > 0; o >>= 1 ) v += __shfl_xor_sync( 0xffffffffu, v, o );
-			return v;
-		}
-		__device__ __forceinline__ float warpMaxF( float v )
-		{
-			for( int o = 16; o > 0; o >>= 1 ) v = fmaxf( v, __shfl_xor_sync( 0xffffffffu, v, o ) );
-			return v;
-		}
-		__device__ __forceinline__ void mmaF( float* c, uint32_t a0, uint32_t a2, uint32_t b0, uint32_t b1 )
-		{
-			// rows 8..15 of the A tile are unused (registers a1, a3 = 0): a unit is 8 weight rows
-			const uint32_t z = 0;
-			asm volatile(
-				"mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-				: "+f"( c[ 0 ] ), "+f"( c[ 1 ] ), "+f"( c[ 2 ] ), "+f"( c[ 3 ] )
-				: "r"( a0 ), "r"( z ), "r"( a2 ), "r"( z ), "r"( b0 ), "r"( b1 ) );
-		}
 		__device__ __forceinline__ void consumerSync() { asm volatile( "bar.sync 1, 256;" ::: "memory" ); }
 
 		// exchange accesses: performed at L2 (gpu scope), never through a possibly stale L1 line
@@ -126,15 +107,9 @@ namespace kern
 			asm volatile( "st.relaxed.gpu.global.u16 [%0], %1;" ::"l"( p ), "h"( b ) : "memory" );
 		}
 		// a protocol bug must not hang the GPU: every wait gives up (trap = launch failure) after ~2 s of wall time
-		__device__ __forceinline__ unsigned long long globalNs()
-		{
-			unsigned long long t;
-			asm volatile( "mov.u64 %0, %globaltimer;" : "=l"( t ) );
-			return t;
-		}
 		__device__ __noinline__ void spinCheck( unsigned long long& t0 )
 		{
-			const unsigned long long t = globalNs();
+			const unsigned long long t = ptx::globaltimer();
 			if( t0 == 0 ) t0 = t;
 			else if( t - t0 > 2000000000ull ) __trap();
 		}
@@ -222,13 +197,6 @@ namespace kern
 			}
 		}
 
-		__device__ __forceinline__ void mmaFull( float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1 )
-		{
-			asm volatile(
-				"mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-				: "+f"( c[ 0 ] ), "+f"( c[ 1 ] ), "+f"( c[ 2 ] ), "+f"( c[ 3 ] )
-				: "r"( a0 ), "r"( a1 ), "r"( a2 ), "r"( a3 ), "r"( b0 ), "r"( b1 ) );
-		}
 		// The 16-byte pieces of a 128-byte K row (or of the query) that lane (g, t) of an MMA holds: pieces t and t + 4, the two swapped
 		// for odd g.  Rows are 128 bytes apart — every row starts in bank 0 — so the eight lanes of a quarter warp (g = 2i, 2i + 1; t = 0..3)
 		// read eight DIFFERENT 16-byte columns in one LDS.128.  A dot product does not care in which order k is walked as long as both
@@ -265,13 +233,13 @@ namespace kern
 					c[ i ][ 0 ] = c[ i ][ 1 ] = c[ i ][ 2 ] = c[ i ][ 3 ] = 0.0f;
 				}
 #pragma unroll
-				for( int i = 0; i < TI; i++ ) mmaFull( c[ i ], a0[ i ].x, b0[ i ].x, a0[ i ].y, b0[ i ].y, qB[ 0 ].x, qB[ 0 ].y );
+				for( int i = 0; i < TI; i++ ) ptx::mma_m16n8k16( c[ i ], a0[ i ].x, b0[ i ].x, a0[ i ].y, b0[ i ].y, qB[ 0 ].x, qB[ 0 ].y );
 #pragma unroll
-				for( int i = 0; i < TI; i++ ) mmaFull( c[ i ], a0[ i ].z, b0[ i ].z, a0[ i ].w, b0[ i ].w, qB[ 0 ].z, qB[ 0 ].w );
+				for( int i = 0; i < TI; i++ ) ptx::mma_m16n8k16( c[ i ], a0[ i ].z, b0[ i ].z, a0[ i ].w, b0[ i ].w, qB[ 0 ].z, qB[ 0 ].w );
 #pragma unroll
-				for( int i = 0; i < TI; i++ ) mmaFull( c[ i ], a1[ i ].x, b1[ i ].x, a1[ i ].y, b1[ i ].y, qB[ 1 ].x, qB[ 1 ].y );
+				for( int i = 0; i < TI; i++ ) ptx::mma_m16n8k16( c[ i ], a1[ i ].x, b1[ i ].x, a1[ i ].y, b1[ i ].y, qB[ 1 ].x, qB[ 1 ].y );
 #pragma unroll
-				for( int i = 0; i < TI; i++ ) mmaFull( c[ i ], a1[ i ].z, b1[ i ].z, a1[ i ].w, b1[ i ].w, qB[ 1 ].z, qB[ 1 ].w );
+				for( int i = 0; i < TI; i++ ) ptx::mma_m16n8k16( c[ i ], a1[ i ].z, b1[ i ].z, a1[ i ].w, b1[ i ].w, qB[ 1 ].z, qB[ 1 ].w );
 				if( ( lane & 3 ) == 0 )
 				{
 #pragma unroll
@@ -290,7 +258,7 @@ namespace kern
 		// softmax over sp[0, n) exactly as the reference does it: max in f32, e = f16-table exp, sum, scale by 1/sum (ggml.c:5026-5095)
 		__device__ __forceinline__ void softmaxRow( float* sp, int n, float lmax, float* sred, int tid, int warp, int lane )
 		{
-			lmax = warpMaxF( lmax );
+			lmax = ptx::warp_max( lmax );
 			if( lane == 0 ) sred[ warp ] = lmax;
 			consumerSync();
 			float mx = sred[ 0 ];
@@ -302,7 +270,7 @@ namespace kern
 				sp[ j ] = e;
 				lsum += e;
 			}
-			lsum = warpSumF( lsum );
+			lsum = ptx::warp_sum( lsum );
 			if( lane == 0 ) sred[ FL_WARPS + warp ] = lsum;   // (the maxima in sred[0..8) may still be being read)
 			consumerSync();
 			float tot = 0.0f;
@@ -394,7 +362,7 @@ namespace kern
 			float s = 0.0f;
 #pragma unroll
 			for( int i = 0; i < N4; i++ ) s += v[ i ].x + v[ i ].y + v[ i ].z + v[ i ].w;
-			const float mean = warpSumF( s ) / (float)D;
+			const float mean = ptx::warp_sum( s ) / (float)D;
 			float sq = 0.0f;
 #pragma unroll
 			for( int i = 0; i < N4; i++ )
@@ -402,7 +370,7 @@ namespace kern
 				v[ i ].x -= mean; v[ i ].y -= mean; v[ i ].z -= mean; v[ i ].w -= mean;
 				sq += v[ i ].x * v[ i ].x + v[ i ].y * v[ i ].y + v[ i ].z * v[ i ].z + v[ i ].w * v[ i ].w;
 			}
-			const float rstd = 1.0f / sqrtf( warpSumF( sq ) / (float)D + 1e-5f );
+			const float rstd = 1.0f / sqrtf( ptx::warp_sum( sq ) / (float)D + 1e-5f );
 			const float4* g4 = reinterpret_cast<const float4*>( gamma );
 			const float4* b4 = reinterpret_cast<const float4*>( beta );
 			uint2* d2 = reinterpret_cast<uint2*>( dst );
@@ -623,7 +591,7 @@ namespace kern
 					if( lane == 0 && pMark < 300 )
 					{
 						a.timing[ 2 * ( 2000 + pMark ) ] = (unsigned long long)( 100000 + 100 * il + code );
-						a.timing[ 2 * ( 2000 + pMark ) + 1 ] = globalNs();
+						a.timing[ 2 * ( 2000 + pMark ) + 1 ] = ptx::globaltimer();
 					}
 					pMark++;
 				};
@@ -749,7 +717,7 @@ namespace kern
 				if( cta == markCta && tid == 0 && markIdx < 2000 )
 				{
 					a.timing[ 2 * markIdx ] = (unsigned long long)id;
-					a.timing[ 2 * markIdx + 1 ] = globalNs();
+					a.timing[ 2 * markIdx + 1 ] = ptx::globaltimer();
 				}
 				markIdx++;
 			};
@@ -1036,13 +1004,13 @@ namespace kern
 										{
 											const uint4 wv = *reinterpret_cast<const uint4*>( wb + st * 64 );
 											const uint4 x0 = *reinterpret_cast<const uint4*>( xb0 + st * 64 );
-											mmaF( acc0[ u ], wv.x, wv.y, x0.x, x0.y );
-											mmaF( acc0[ u ], wv.z, wv.w, x0.z, x0.w );
+											ptx::mma_m16n8k16_rows8( acc0[ u ], wv.x, wv.y, x0.x, x0.y );
+											ptx::mma_m16n8k16_rows8( acc0[ u ], wv.z, wv.w, x0.z, x0.w );
 											if( twoTiles )
 											{
 												const uint4 x1v = *reinterpret_cast<const uint4*>( xb1 + st * 64 );
-												mmaF( acc1[ u ], wv.x, wv.y, x1v.x, x1v.y );
-												mmaF( acc1[ u ], wv.z, wv.w, x1v.z, x1v.w );
+												ptx::mma_m16n8k16_rows8( acc1[ u ], wv.x, wv.y, x1v.x, x1v.y );
+												ptx::mma_m16n8k16_rows8( acc1[ u ], wv.z, wv.w, x1v.z, x1v.w );
 											}
 										}
 									}

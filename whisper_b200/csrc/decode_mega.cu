@@ -31,51 +31,14 @@ namespace kern
 		constexpr int MG_SMEM_PARAM = 2 * 1280 * 4 + 8 * MG_ROWS * 4;   // LayerNorm gamma | beta of the next phase + biases of this CTA's units
 		constexpr int MG_MAXBIASUNITS = 8;
 
-		__device__ __forceinline__ float warpSumM( float v )
-		{
-			for( int o = 16; o > 0; o >>= 1 ) v += __shfl_xor_sync( 0xffffffffu, v, o );
-			return v;
-		}
-		__device__ __forceinline__ float warpMaxM( float v )
-		{
-			for( int o = 16; o > 0; o >>= 1 ) v = fmaxf( v, __shfl_xor_sync( 0xffffffffu, v, o ) );
-			return v;
-		}
-		__device__ __forceinline__ void mmaM( float* c, uint32_t a0, uint32_t a2, uint32_t b0, uint32_t b1 )
-		{
-			// rows 8..15 of the A tile are unused (registers a1, a3 = 0): a unit is 8 weight rows
-			const uint32_t z = 0;
-			asm volatile(
-				"mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-				: "+f"( c[ 0 ] ), "+f"( c[ 1 ] ), "+f"( c[ 2 ] ), "+f"( c[ 3 ] )
-				: "r"( a0 ), "r"( z ), "r"( a2 ), "r"( z ), "r"( b0 ), "r"( b1 ) );
-		}
-		__device__ __forceinline__ uint4 ldgStream( const uint4* p )
-		{
-			uint4 r;
-			asm volatile( "ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"( r.x ), "=r"( r.y ), "=r"( r.z ), "=r"( r.w ) : "l"( p ) );
-			return r;
-		}
 		// data written by other CTAs earlier in this launch: read at L2 (never through a possibly stale L1 line)
 		__device__ __forceinline__ float4 ldcg4( const float* p ) { return __ldcg( reinterpret_cast<const float4*>( p ) ); }
 		__device__ __forceinline__ uint4 ldcgU4( const void* p ) { return __ldcg( reinterpret_cast<const uint4*>( p ) ); }
 
-		__device__ __forceinline__ void cpAsync16( void* smemDst, const void* gmemSrc )
-		{
-			asm volatile( "cp.async.cg.shared.global [%0], [%1], 16;" ::"r"( ptx::smem_u32( smemDst ) ), "l"( gmemSrc ) : "memory" );
-		}
-		__device__ __forceinline__ void cpAsyncCommit() { asm volatile( "cp.async.commit_group;" ::: "memory" ); }
-		__device__ __forceinline__ void cpAsyncWaitAll() { asm volatile( "cp.async.wait_group 0;" ::: "memory" ); }
-
 		// debug: CTA 0 / thread 0 writes %globaltimer into a fixed slot (last layer wins); tm == nullptr in normal runs
 		__device__ __forceinline__ void subMark( unsigned long long* tm, int k )
 		{
-			if( tm && threadIdx.x == 0 )
-			{
-				unsigned long long t;
-				asm volatile( "mov.u64 %0, %globaltimer;" : "=l"( t ) );
-				tm[ k ] = t;
-			}
+			if( tm && threadIdx.x == 0 ) tm[ k ] = ptx::globaltimer();
 		}
 
 		struct Smem
@@ -112,12 +75,7 @@ namespace kern
 					asm volatile( "atom.add.release.gpu.global.u32 %0, [%1], 1;" : "=r"( old ) : "l"( counter ) : "memory" );
 					if( old == target - 1 )
 						asm volatile( "st.release.gpu.global.u32 [%0], %1;" ::"l"( counter + 32 ), "r"( epoch ) : "memory" );
-					if( tm )
-					{
-						unsigned long long t;
-						asm volatile( "mov.u64 %0, %globaltimer;" : "=l"( t ) );
-						tm[ 5 ] = t;
-					}
+					if( tm ) tm[ 5 ] = ptx::globaltimer();
 				}
 			}
 			__device__ __forceinline__ void wait()
@@ -197,7 +155,7 @@ namespace kern
 				{
 					const int st = warp + MG_WARPS * ( sub * S::SUB + s );
 					if( ui < nMine && st < S::STEPS )
-						wb.w[ u * S::SUB + s ] = ldgStream( wr + st * 4 );
+						wb.w[ u * S::SUB + s ] = ptx::ldg_stream( wr + st * 4 );
 				}
 			}
 		}
@@ -214,8 +172,8 @@ namespace kern
 				const int n16 = K / 4;   // 16-byte chunks per vector
 				for( int i = tid; i < 2 * n16; i += MG_THREADS )
 				{
-					if( i < n16 ) cpAsync16( sm.gamma + i * 4, op.gamma + i * 4 );
-					else cpAsync16( sm.beta + ( i - n16 ) * 4, op.beta + ( i - n16 ) * 4 );
+					if( i < n16 ) ptx::cp_async16( sm.gamma + i * 4, op.gamma + i * 4 );
+					else ptx::cp_async16( sm.beta + ( i - n16 ) * 4, op.beta + ( i - n16 ) * 4 );
 				}
 			}
 			if( op.bias )
@@ -226,10 +184,10 @@ namespace kern
 					const int ui = tid >> 1, half = tid & 1;
 					const int unit = blockIdx.x + ui * gridDim.x;
 					if( unit < units && unit * MG_ROWS + half * 4 + 4 <= op.nOut )
-						cpAsync16( sm.bias + ui * MG_ROWS + half * 4, op.bias + unit * MG_ROWS + half * 4 );
+						ptx::cp_async16( sm.bias + ui * MG_ROWS + half * 4, op.bias + unit * MG_ROWS + half * 4 );
 				}
 			}
-			cpAsyncCommit();
+			ptx::cp_async_commit();
 		}
 
 		template<int K>
@@ -265,7 +223,7 @@ namespace kern
 					v[ i ] = ldcg4( src + ( i * 32 + lane ) * 4 );
 					s += v[ i ].x + v[ i ].y + v[ i ].z + v[ i ].w;
 				}
-				const float mean = warpSumM( s ) / (float)K;
+				const float mean = ptx::warp_sum( s ) / (float)K;
 				float sq = 0.0f;
 #pragma unroll
 				for( int i = 0; i < N4; i++ )
@@ -273,7 +231,7 @@ namespace kern
 					v[ i ].x -= mean; v[ i ].y -= mean; v[ i ].z -= mean; v[ i ].w -= mean;
 					sq += v[ i ].x * v[ i ].x + v[ i ].y * v[ i ].y + v[ i ].z * v[ i ].z + v[ i ].w * v[ i ].w;
 				}
-				const float rstd = 1.0f / sqrtf( warpSumM( sq ) / (float)K + 1e-5f );
+				const float rstd = 1.0f / sqrtf( ptx::warp_sum( sq ) / (float)K + 1e-5f );
 				const float4* g4 = reinterpret_cast<const float4*>( sm.gamma );
 				const float4* b4 = reinterpret_cast<const float4*>( sm.beta );
 				uint2* d2 = reinterpret_cast<uint2*>( dst );
@@ -377,13 +335,13 @@ namespace kern
 							{
 								const uint4 w = wb.w[ u * S::SUB + s ];
 								const uint4 x0 = *reinterpret_cast<const uint4*>( xb0 + st * 32 );
-								mmaM( acc0[ u ], w.x, w.y, x0.x, x0.y );
-								mmaM( acc0[ u ], w.z, w.w, x0.z, x0.w );
+								ptx::mma_m16n8k16_rows8( acc0[ u ], w.x, w.y, x0.x, x0.y );
+								ptx::mma_m16n8k16_rows8( acc0[ u ], w.z, w.w, x0.z, x0.w );
 								if( twoTiles )
 								{
 									const uint4 x1 = *reinterpret_cast<const uint4*>( xb1 + st * 32 );
-									mmaM( acc1[ u ], w.x, w.y, x1.x, x1.y );
-									mmaM( acc1[ u ], w.z, w.w, x1.z, x1.w );
+									ptx::mma_m16n8k16_rows8( acc1[ u ], w.x, w.y, x1.x, x1.y );
+									ptx::mma_m16n8k16_rows8( acc1[ u ], w.z, w.w, x1.z, x1.w );
 								}
 							}
 						}
@@ -445,8 +403,8 @@ namespace kern
 				const bool isV = i >= n;
 				const int k = isV ? i - n : i;
 				const int j = j0 + ( k >> 3 ), c = k & 7;
-				if( isV ) cpAsync16( sV + j * 128 + c * 16, vb + (size_t)j * 64 + c * 8 );
-				else cpAsync16( sK + j * SA_KSTRIDE + c * 16, kb + (size_t)j * 64 + c * 8 );
+				if( isV ) ptx::cp_async16( sV + j * 128 + c * 16, vb + (size_t)j * 64 + c * 8 );
+				else ptx::cp_async16( sK + j * SA_KSTRIDE + c * 16, kb + (size_t)j * 64 + c * 8 );
 			}
 		}
 		__device__ void selfAttnPhase( const MegaArgs& a, const MegaLayer& L, int d, int nPast, const Smem& sm, int warp, int lane, int tid )
@@ -464,10 +422,10 @@ namespace kern
 				const int b = unit / H, h = unit - b * H;
 				// rows [0, nkv-1) of the first unit were requested before the barrier; the new row (and everything for further units) now
 				selfLoadRows( a, L, d, sm, unit, first ? nkv - 1 : 0, nkv, tid );
-				cpAsyncCommit();
+				ptx::cp_async_commit();
 				first = false;
 				if( tid < 64 ) sq[ tid ] = __half2float( __float2half_rn( __ldcg( a.q + (size_t)b * d + h * 64 + tid ) ) );
-				cpAsyncWaitAll();
+				ptx::cp_async_wait_all();
 				__syncthreads();
 				float lmax = -INFINITY;
 				for( int j = tid; j < nkv; j += MG_THREADS )
@@ -489,7 +447,7 @@ namespace kern
 					sm.sp[ j ] = s;
 					lmax = fmaxf( lmax, s );
 				}
-				lmax = warpMaxM( lmax );
+				lmax = ptx::warp_max( lmax );
 				if( lane == 0 ) sred[ warp ] = lmax;
 				__syncthreads();
 				float mx = sred[ 0 ];
@@ -502,7 +460,7 @@ namespace kern
 					sm.sp[ j ] = e;
 					lsum += e;
 				}
-				lsum = warpSumM( lsum );
+				lsum = ptx::warp_sum( lsum );
 				if( lane == 0 ) sred[ warp ] = lsum;
 				__syncthreads();
 				float tot = 0.0f;
@@ -555,8 +513,8 @@ namespace kern
 			const uint4* V4 = reinterpret_cast<const uint4*>( L.crossV + base );
 			const uint4* K4 = reinterpret_cast<const uint4*>( L.crossK + base );
 			uint4* sv = reinterpret_cast<uint4*>( sm.a );
-			for( int idx = tid; idx < T * 8; idx += MG_THREADS ) cpAsync16( sv + idx, V4 + idx );
-			cpAsyncCommit();
+			for( int idx = tid; idx < T * 8; idx += MG_THREADS ) ptx::cp_async16( sv + idx, V4 + idx );
+			ptx::cp_async_commit();
 			const int sub = lane & 7, rgrp = lane >> 3;
 			const int jb = warp * 4 + rgrp;
 #pragma unroll
@@ -620,7 +578,7 @@ namespace kern
 						}
 					}
 				}
-				lmax = warpMaxM( lmax );
+				lmax = ptx::warp_max( lmax );
 				if( lane == 0 ) sred[ warp ] = lmax;
 				__syncthreads();
 				float mx = sred[ 0 ];
@@ -633,14 +591,14 @@ namespace kern
 					sm.sp[ j ] = e;
 					lsum += e;
 				}
-				lsum = warpSumM( lsum );
+				lsum = ptx::warp_sum( lsum );
 				if( lane == 0 ) sred[ warp ] = lsum;
 				__syncthreads();
 				float tot = 0.0f;
 				for( int w = 0; w < MG_WARPS; w++ ) tot += sred[ w ];
 				const float inv = 1.0f / tot;
 				for( int j = tid; j < T; j += MG_THREADS ) sm.sp[ j ] *= inv;
-				cpAsyncWaitAll();
+				ptx::cp_async_wait_all();
 				__syncthreads();
 				const __half* sv = reinterpret_cast<const __half*>( sm.a );
 				const int parts = a.refThreads > 0 ? a.refThreads : 4;
@@ -693,8 +651,7 @@ namespace kern
 			auto markId = [ & ]( int id ) {
 				if( a.timing && blockIdx.x == 0 && tid == 0 && markIdx < 2040 )
 				{
-					unsigned long long t;
-					asm volatile( "mov.u64 %0, %globaltimer;" : "=l"( t ) );
+					const unsigned long long t = ptx::globaltimer();
 					a.timing[ 2 * markIdx ] = (unsigned long long)id;
 					a.timing[ 2 * markIdx + 1 ] = t;
 				}
@@ -757,7 +714,7 @@ namespace kern
 				prefetchParams( o, D, sm, tid );
 			};
 			// after the barrier: parameters have landed
-			auto landed = [ & ]() { cpAsyncWaitAll(); __syncthreads(); };
+			auto landed = [ & ]() { ptx::cp_async_wait_all(); __syncthreads(); };
 
 			// a layer's cross-attention K/V tile of "my" (chunk, head) starts moving HBM -> L2 several phases ahead of its use (those
 			// phases are latency-bound and leave the DRAM pipe idle); issued while waiting at a barrier, off the critical path
@@ -850,7 +807,7 @@ namespace kern
 					{
 						// earlier tokens' K/V rows of my (chunk, head) -> smem (region A is free: the activations are consumed)
 						selfLoadRows( a, L, D, sm, blockIdx.x, 0, nkvOld, tid );
-						cpAsyncCommit();
+						ptx::cp_async_commit();
 					}
 					else if( ph == PH_CQ )
 						crossPrefetch( a, L, pf, sm, blockIdx.x, warp, lane, tid );   // V tile -> smem (region A is free now), first K rows -> registers

@@ -38,6 +38,7 @@ namespace wsp
 	constexpr int kConv1KTap = 128;        // 80 input channels padded to two 64-wide K blocks per tap
 	constexpr int kMaxDecodeTokens = 256;  // tokens per chunk in one decoder call (prompt <= 224 + 4)
 	constexpr int kAllLogitsTokens = 8;
+	constexpr int kStepMarks = 4608;       // 64-bit debug marks the decoder-step kernels may write (wsp_debug_step_timing)
 
 	struct LnW { float* g = nullptr; float* b = nullptr; };
 	struct EncLayerW
@@ -165,17 +166,17 @@ namespace wsp
 		// persistent decoder-step kernel (decode_mega.cu): per-layer pointer table on the device, grid-barrier counter
 		kern::MegaLayer* megaLayers = nullptr;
 		unsigned* megaBarrier = nullptr;
-		unsigned long long* megaTiming = nullptr;   // [4096] debug marks
 		// dataflow decoder-step kernel (decode_flow.cu): per-layer pointer table, per-CTA bias slabs, exchange buffers, launch epoch
 		kern::FlowLayer* flowLayers = nullptr;
 		float* flowBias = nullptr;
 		uint8_t* flowExch = nullptr;
 		unsigned* flowCtrl = nullptr;
 		kern::FlowGeom flowGeom;
-		// N = 1 decoder step: 2 = dataflow kernel (default), 1 = round 1's barrier kernel, 0 = one kernel per op
+		// N = 1 decoder step (wsp_debug_set_step_mode): 2 = dataflow kernel (default), 1 = round 1's barrier kernel, 0 = one kernel per op
 		int stepMode = 2;
-		int stepTimingCta = 0;
-		bool stepTiming = false;        // record %globaltimer marks of CTA 0 into megaTiming (wsp_debug_step_timing)
+		unsigned long long* stepMarks = nullptr;   // [kStepMarks] debug marks of the step kernels, read by wsp_debug_step_timing
+		bool stepTiming = false;        // the step kernels record %globaltimer marks into stepMarks (wsp_debug_enable_step_timing)
+		int stepTimingCta = 0;          // CTA whose marks the dataflow kernel records (WSP_TIMING_CTA; the barrier kernel's is CTA 0)
 
 		// decode CUDA graph (N = 1 steady state)
 		cudaGraphExec_t stepGraph = nullptr;

@@ -8,8 +8,7 @@
 namespace kern
 {
 	// Launch with the programmatic-stream-serialization attribute (PDL).  Kernels launched this way call pdl_launch_dependents() first
-	// thing and pdl_wait() before touching anything a predecessor wrote.  WSP_PDL=0 in the environment disables the attribute.
-	bool pdlEnabled();
+	// thing and pdl_wait() before touching anything a predecessor wrote.
 	template<class... KArgs, class... Args>
 	inline cudaError_t launchPdl( void ( *kernel )( KArgs... ), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args )
 	{
@@ -22,7 +21,7 @@ namespace kern
 		at[ 0 ].id = cudaLaunchAttributeProgrammaticStreamSerialization;
 		at[ 0 ].val.programmaticStreamSerializationAllowed = 1;
 		cfg.attrs = at;
-		cfg.numAttrs = pdlEnabled() ? 1 : 0;
+		cfg.numAttrs = 1;
 		return cudaLaunchKernelEx( &cfg, kernel, static_cast<KArgs>( args )... );
 	}
 
@@ -122,9 +121,9 @@ namespace kern
 		int* history = nullptr;         // optional [B][histCap] token log, written at column *dStep
 		int histCap = 0;
 		int* dStep = nullptr;
-		int rowInSmem = 0;              // set by sampleGreedy: the row fits the 227 KB shared memory
-		int* tieScratch = nullptr;      // [B][nVocab + 1024] ints: survivor lists of the exact tie emulation (null: one-thread emulation)
+		int* tieScratch = nullptr;      // required: [B][nVocab + 1024] ints, survivor lists of the exact tie emulation
 	};
+	// one cluster of 4 CTAs per row (any nVocab >= 8 whose quarter fits shared memory), then the 1-thread advance of n_past / flags / step
 	cudaError_t sampleGreedy( const SampleArgs& a, cudaStream_t s );
 
 	// row-wise softmax of [rows][n] (all-logits test mode)

@@ -5,21 +5,9 @@
 #include "ref_arith.cuh"
 #include <math.h>
 #include <cooperative_groups.h>
-#include <stdlib.h>
 
 namespace kern
 {
-	__device__ __forceinline__ float warpSumD( float v )
-	{
-		for( int o = 16; o > 0; o >>= 1 ) v += __shfl_xor_sync( 0xffffffffu, v, o );
-		return v;
-	}
-	__device__ __forceinline__ float warpMaxD( float v )
-	{
-		for( int o = 16; o > 0; o >>= 1 ) v = fmaxf( v, __shfl_xor_sync( 0xffffffffu, v, o ) );
-		return v;
-	}
-
 	// ---------------------------------------------------------------------------------------------------------------
 	// Skinny GEMM: out[col][n] = sum_k W[n][k] * x[col][k] for a handful of columns (decoder tokens x chunks).
 	//
@@ -35,21 +23,6 @@ namespace kern
 	constexpr int SK_COLS = 16;      // columns per CTA pass (2 n-tiles of 8)
 	constexpr int SK_WARPS = 8;
 	constexpr int SK_PAD = 32;       // halves of padding per activation row: row stride = 64 (mod 128) bytes -> conflict-free LDS.128
-
-	__device__ __forceinline__ void mma16816( float* c, const uint32_t* a, uint32_t b0, uint32_t b1 )
-	{
-		asm volatile(
-			"mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-			: "+f"( c[ 0 ] ), "+f"( c[ 1 ] ), "+f"( c[ 2 ] ), "+f"( c[ 3 ] )
-			: "r"( a[ 0 ] ), "r"( a[ 1 ] ), "r"( a[ 2 ] ), "r"( a[ 3 ] ), "r"( b0 ), "r"( b1 ) );
-	}
-
-	__device__ __forceinline__ uint4 ldg_stream( const uint4* p )
-	{
-		uint4 r;
-		asm volatile( "ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"( r.x ), "=r"( r.y ), "=r"( r.z ), "=r"( r.w ) : "l"( p ) );
-		return r;
-	}
 
 	__global__ void __launch_bounds__( SK_WARPS * 32 )
 		skinny_gemm_kernel( SkinnyArgs a )
@@ -84,8 +57,8 @@ namespace kern
 			const int st = warp + u * SK_WARPS;
 			if( st < steps )
 			{
-				va[ u ] = ldg_stream( wA + st * 4 );   // 32 halves = 4 uint4 per step
-				vb[ u ] = ldg_stream( wB + st * 4 );
+				va[ u ] = ptx::ldg_stream( wA + st * 4 );   // 32 halves = 4 uint4 per step
+				vb[ u ] = ptx::ldg_stream( wB + st * 4 );
 			}
 		}
 
@@ -125,7 +98,7 @@ namespace kern
 							v[ q4 ] = s4[ q4 * 32 + lane ];
 							s += v[ q4 ].x + v[ q4 ].y + v[ q4 ].z + v[ q4 ].w;
 						}
-					const float mean = warpSumD( s ) / (float)K;
+					const float mean = ptx::warp_sum( s ) / (float)K;
 					float sq = 0.0f;
 #pragma unroll
 					for( int q4 = 0; q4 < MAXV; q4++ )
@@ -134,7 +107,7 @@ namespace kern
 							v[ q4 ].x -= mean; v[ q4 ].y -= mean; v[ q4 ].z -= mean; v[ q4 ].w -= mean;
 							sq += v[ q4 ].x * v[ q4 ].x + v[ q4 ].y * v[ q4 ].y + v[ q4 ].z * v[ q4 ].z + v[ q4 ].w * v[ q4 ].w;
 						}
-					const float rstd = 1.0f / sqrtf( warpSumD( sq ) / (float)K + 1e-5f );
+					const float rstd = 1.0f / sqrtf( ptx::warp_sum( sq ) / (float)K + 1e-5f );
 					const float4* g4 = reinterpret_cast<const float4*>( a.gamma );
 					const float4* b4 = reinterpret_cast<const float4*>( a.beta );
 					uint2* d2 = reinterpret_cast<uint2*>( dst );
@@ -178,15 +151,13 @@ namespace kern
 				if( st < steps )
 				{
 					const uint4 x0 = *reinterpret_cast<const uint4*>( xb0 + st * 32 );
-					const uint32_t a1[ 4 ] = { va[ u ].x, vb[ u ].x, va[ u ].y, vb[ u ].y };
-					const uint32_t a2[ 4 ] = { va[ u ].z, vb[ u ].z, va[ u ].w, vb[ u ].w };
-					mma16816( acc0, a1, x0.x, x0.y );
-					mma16816( acc0, a2, x0.z, x0.w );
+					ptx::mma_m16n8k16( acc0, va[ u ].x, vb[ u ].x, va[ u ].y, vb[ u ].y, x0.x, x0.y );
+					ptx::mma_m16n8k16( acc0, va[ u ].z, vb[ u ].z, va[ u ].w, vb[ u ].w, x0.z, x0.w );
 					if( twoTiles )
 					{
 						const uint4 x1 = *reinterpret_cast<const uint4*>( xb1 + st * 32 );
-						mma16816( acc1, a1, x1.x, x1.y );
-						mma16816( acc1, a2, x1.z, x1.w );
+						ptx::mma_m16n8k16( acc1, va[ u ].x, vb[ u ].x, va[ u ].y, vb[ u ].y, x1.x, x1.y );
+						ptx::mma_m16n8k16( acc1, va[ u ].z, vb[ u ].z, va[ u ].w, vb[ u ].w, x1.z, x1.w );
 					}
 				}
 			}
@@ -199,8 +170,8 @@ namespace kern
 					const int st = s0 + u * SK_WARPS;
 					if( st < steps )
 					{
-						va[ u ] = ldg_stream( wA + st * 4 );
-						vb[ u ] = ldg_stream( wB + st * 4 );
+						va[ u ] = ptx::ldg_stream( wA + st * 4 );
+						vb[ u ] = ptx::ldg_stream( wB + st * 4 );
 					}
 				}
 			}
@@ -338,7 +309,7 @@ namespace kern
 			sp[ j ] = s;
 			lmax = fmaxf( lmax, s );
 		}
-		lmax = warpMaxD( lmax );
+		lmax = ptx::warp_max( lmax );
 		if( ( tid & 31 ) == 0 ) sred[ tid >> 5 ] = lmax;
 		__syncthreads();
 		float mx = sred[ 0 ];
@@ -351,7 +322,7 @@ namespace kern
 			sp[ j ] = e;
 			lsum += e;
 		}
-		lsum = warpSumD( lsum );
+		lsum = ptx::warp_sum( lsum );
 		if( ( tid & 31 ) == 0 ) sred[ tid >> 5 ] = lsum;
 		__syncthreads();
 		float tot = 0.0f;
@@ -405,13 +376,6 @@ namespace kern
 	constexpr int CA_MAXT = 1536;
 	constexpr int CA_UNROLL = 12;
 
-	__device__ __forceinline__ void cp_async16( void* smemDst, const void* gmemSrc )
-	{
-		asm volatile( "cp.async.cg.shared.global [%0], [%1], 16;" ::"r"( ptx::smem_u32( smemDst ) ), "l"( gmemSrc ) : "memory" );
-	}
-	__device__ __forceinline__ void cp_async_commit() { asm volatile( "cp.async.commit_group;" ::: "memory" ); }
-	__device__ __forceinline__ void cp_async_wait_all() { asm volatile( "cp.async.wait_group 0;" ::: "memory" ); }
-
 	__global__ void __launch_bounds__( CA_THREADS )
 		cross_attn_decode_kernel( const float* __restrict__ q, const __half* __restrict__ kMem, const __half* __restrict__ vMem, __half* __restrict__ out,
 			int N, int H, int d, int T, int refThreads )
@@ -435,8 +399,8 @@ namespace kern
 		// kernel (the cross-KV memories were written by the encoder), so both prefetches are issued before the dependency wait.
 		{
 			uint4* sv = reinterpret_cast<uint4*>( ca_smem );
-			for( int idx = tid; idx < T * 8; idx += CA_THREADS ) cp_async16( sv + idx, V4 + idx );
-			cp_async_commit();
+			for( int idx = tid; idx < T * 8; idx += CA_THREADS ) ptx::cp_async16( sv + idx, V4 + idx );
+			ptx::cp_async_commit();
 		}
 		constexpr int JSTEP = ( CA_THREADS / 32 ) * 4;
 		int jb = warp * 4 + rgrp;
@@ -490,7 +454,7 @@ namespace kern
 				}
 			}
 		}
-		lmax = warpMaxD( lmax );
+		lmax = ptx::warp_max( lmax );
 		if( lane == 0 ) sred[ warp ] = lmax;
 		__syncthreads();
 		float mx = sred[ 0 ];
@@ -503,14 +467,14 @@ namespace kern
 			sp[ j ] = e;
 			lsum += e;
 		}
-		lsum = warpSumD( lsum );
+		lsum = ptx::warp_sum( lsum );
 		if( lane == 0 ) sred[ warp ] = lsum;
 		__syncthreads();
 		float tot = 0.0f;
 		for( int w = 0; w < CA_THREADS / 32; w++ ) tot += sred[ w ];
 		const float inv = 1.0f / tot;
 		for( int j = tid; j < T; j += CA_THREADS ) sp[ j ] *= inv;   // normalised P (ggml.c:5085-5090)
-		cp_async_wait_all();
+		ptx::cp_async_wait_all();
 		__syncthreads();
 
 		const __half* sv = reinterpret_cast<const __half*>( ca_smem );
@@ -578,14 +542,14 @@ namespace kern
 	}
 
 	// ---------------------------------------------------------------------------------------------------------------
-	// softmax over the vocabulary + greedy sampling with the timestamp rules, one CTA per chunk.
+	// softmax over the vocabulary + greedy sampling with the timestamp rules, one cluster of 4 CTAs per chunk.
 	// Oracle: ggml_soft_max (ggml.c:5026-5095) then whisper_sample_best (whisper.cpp:1875-1964):
 	//   max_tx = max p(text); if is_initial: p(ts > beg+100) = -inf; sum_ts, max_ts/tid over timestamp tokens;
 	//   if sum_ts > max_tx or force_timestamp: p(text) = -inf;  top-4 by p; skip sot/solm/not among the first three.
 	constexpr int SM_THREADS = 1024;
 
 	// arg-max candidate; `tie`: another token has exactly the same probability (then the reference's pick depends on how
-	// std::partial_sort happens to arrange equal keys, see emulatePartialSort)
+	// std::partial_sort happens to arrange equal keys, see emulatePartialSortCta)
 	struct Top1 { float v; int i; int tie; };
 	__device__ __forceinline__ Top1 better( Top1 a, Top1 b )
 	{
@@ -597,8 +561,8 @@ namespace kern
 	// The reference ranks candidates with std::partial_sort( top 4 ) on (probability, id) pairs compared by probability only
 	// (whisper.cpp:1932-1941).  With distinct probabilities that is "the largest"; with EXACT ties — typically a whole range of
 	// probabilities that underflowed to 0 in the f16-table softmax — the winner is whatever libstdc++'s heap-select + sort-heap leaves
-	// first.  This is that algorithm, statement by statement (bits/stl_heap.h: __push_heap, __adjust_heap, __make_heap, __sort_heap;
-	// bits/stl_algo.h: __heap_select), run by ONE thread over the row: slow (~1 ms) and only entered when a tie decides the token.
+	// first.  emulatePartialSortCta replays that algorithm, statement by statement (bits/stl_heap.h: __push_heap, __adjust_heap,
+	// __make_heap, __sort_heap; bits/stl_algo.h: __heap_select), and is only entered when a tie decides the token.
 	struct ProbId { double v; int i; };
 	__device__ void heapPush( ProbId* f, int hole, int top, ProbId val )
 	{
@@ -630,46 +594,13 @@ namespace kern
 		}
 		heapPush( f, hole, top, val );
 	}
-	__device__ __noinline__ Top1 emulatePartialSort( const float* probs, int nv, int beg, bool maskText, bool isInitial, int sot, int solm, int nott )
-	{
-		auto val = [ & ]( int i, float p ) -> double {
-			if( ( maskText && i < beg ) || ( isInitial && i >= beg + 101 ) ) return -(double)INFINITY;
-			return (double)p;
-		};
-		ProbId f[ 4 ];
-		for( int k = 0; k < 4; k++ ) f[ k ] = ProbId{ val( k, __ldcg( probs + k ) ), k };
-		// __make_heap( first, first + 4 )
-		for( int parent = ( 4 - 2 ) / 2;; parent-- )
-		{
-			const ProbId v = f[ parent ];
-			heapAdjust( f, parent, 4, v );
-			if( parent == 0 ) break;
-		}
-		// __heap_select: every later element that compares before the root replaces it
-		for( int i = 4; i < nv; i++ )
-		{
-			const double v = val( i, __ldcg( probs + i ) );
-			if( v > f[ 0 ].v ) heapAdjust( f, 0, 4, ProbId{ v, i } );
-		}
-		// __sort_heap
-		for( int last = 3; last >= 1; last-- )
-		{
-			const ProbId v = f[ last ];
-			f[ last ] = f[ 0 ];
-			heapAdjust( f, 0, last, v );
-		}
-		int res = 0;
-		while( ( f[ res ].i == sot || f[ res ].i == solm || f[ res ].i == nott ) && res < 3 ) res++;
-		return Top1{ (float)f[ res ].v, f[ res ].i, 0 };
-	}
 
-	// The same result with the whole CTA at work.  std::__heap_select only ever moves an element into the heap that compares
+	// The whole CTA at work on one row.  std::__heap_select only ever moves an element into the heap that compares
 	// strictly above the heap's root, and the root — the 4th largest value of the prefix processed so far — never decreases.  So
 	// after thread 0 has run the exact algorithm over the first TIE_PRE elements, every later element that is not above the root
 	// reached there (T1) can be dropped without changing a single heap operation: all warps filter their contiguous region of the row
 	// against T1 (coalesced loads, ballot, survivors appended in index order to `scratch`), and thread 0 replays the exact algorithm
-	// over the survivors only.  A row whose top probability is shared is far cheaper this way than on one thread
-	// (degenerate rows tie at every step).  Called by every thread of the CTA; the result is valid
+	// over the survivors only, which keeps degenerate rows (they tie at every step) cheap.  Called by every thread of the CTA; the result is valid
 	// in thread 0.  scratch: nv + 32 * warps ints.
 	constexpr int TIE_PRE = 1024;
 	struct TieShared
@@ -690,12 +621,14 @@ namespace kern
 		if( tid == 0 )
 		{
 			for( int k = 0; k < 4; k++ ) f[ k ] = ProbId{ val( k, __ldcg( probs + k ) ), k };
+			// __make_heap( first, first + 4 )
 			for( int parent = ( 4 - 2 ) / 2;; parent-- )
 			{
 				const ProbId v = f[ parent ];
 				heapAdjust( f, parent, 4, v );
 				if( parent == 0 ) break;
 			}
+			// __heap_select: every later element that compares before the root replaces it
 			for( int i = 4; i < pre; i++ )
 			{
 				const double v = val( i, __ldcg( probs + i ) );
@@ -770,19 +703,9 @@ namespace kern
 		for( int w = 1; w < SM_THREADS / 32; w++ ) r = better( r, sbuf[ w ] );
 		return r;
 	}
-	__device__ float blockSumF( float v, float* sbuf )
-	{
-		v = warpSumD( v );
-		__syncthreads();
-		if( ( threadIdx.x & 31 ) == 0 ) sbuf[ threadIdx.x >> 5 ] = v;
-		__syncthreads();
-		float r = 0.0f;
-		for( int w = 0; w < SM_THREADS / 32; w++ ) r += sbuf[ w ];
-		return r;
-	}
 	__device__ float blockMaxF( float v, float* sbuf )
 	{
-		v = warpMaxD( v );
+		v = ptx::warp_max( v );
 		__syncthreads();
 		if( ( threadIdx.x & 31 ) == 0 ) sbuf[ threadIdx.x >> 5 ] = v;
 		__syncthreads();
@@ -792,7 +715,7 @@ namespace kern
 	}
 	__device__ double blockSumD( double v, double* sbuf )
 	{
-		for( int o = 16; o > 0; o >>= 1 ) v += __shfl_xor_sync( 0xffffffffu, v, o );
+		v = ptx::warp_sum( v );
 		__syncthreads();
 		if( ( threadIdx.x & 31 ) == 0 ) sbuf[ threadIdx.x >> 5 ] = v;
 		__syncthreads();
@@ -822,105 +745,14 @@ namespace kern
 		if( threadIdx.x == 0 ) sh.tie = needsTieEmulation( pick, a, probsRow, maskText ) ? 1 : 0;
 		__syncthreads();
 		if( !sh.tie ) return pick;
-		if( !a.tieScratch )
-		{
-			if( threadIdx.x == 0 ) pick = emulatePartialSort( probsRow, a.nVocab, a.tokenBeg, maskText, isInitial, a.tokenSot, a.tokenSolm, a.tokenNot );
-			return pick;
-		}
 		const Top1 r = emulatePartialSortCta( probsRow, a.nVocab, a.tokenBeg, maskText, isInitial, a.tokenSot, a.tokenSolm, a.tokenNot,
 			a.tieScratch + (size_t)b * ( a.nVocab + 32 * ( SM_THREADS / 32 ) ), sh, SM_THREADS );
 		return threadIdx.x == 0 ? r : pick;
 	}
 
-	__global__ void __launch_bounds__( SM_THREADS )
-		sample_kernel( SampleArgs a )
-	{
-		__shared__ float sf[ SM_THREADS / 32 ];
-		__shared__ double sd[ SM_THREADS / 32 ];
-		__shared__ Top1 st[ SM_THREADS / 32 ];
-		ptx::pdl_launch_dependents();
-		ptx::pdl_wait();
-		const int b = blockIdx.x;
-		const int tid = threadIdx.x;
-		const int nv = a.nVocab;
-		const float* lg = a.logits + (size_t)b * nv;
-		float* gpr = a.probs + (size_t)b * nv;
-		// the row lives in shared memory when it fits (207 KB for 51865 tokens): its seven passes then read shared memory instead of L2
-		extern __shared__ float sampleRow[];
-		float* pr = a.rowInSmem ? sampleRow : gpr;
-		const bool forceTs = a.dForceTs && a.dForceTs[ 0 ] != 0;
-		const bool isInitial = a.dForceTs && a.dForceTs[ 1 ] != 0;
-
-		float mx = -INFINITY;
-		for( int i = tid; i < nv; i += SM_THREADS )
-		{
-			const float v = __ldcg( lg + i );
-			pr[ i ] = v;
-			mx = fmaxf( mx, v );
-		}
-		mx = blockMaxF( mx, sf );
-		double dsum = 0.0;
-		for( int i = tid; i < nv; i += SM_THREADS )
-		{
-			const float e = expF16Table( pr[ i ] - mx );
-			pr[ i ] = e;
-			dsum += (double)e;
-		}
-		dsum = blockSumD( dsum, sd );
-		const float inv = (float)( 1.0 / dsum );
-		// timestamp bookkeeping on the normalised probabilities
-		const int beg = a.tokenBeg;
-		const int tsEnd = isInitial ? min( beg + 101, nv ) : nv;   // initial timestamp <= 1 s (whisper.cpp:1902-1911)
-		float maxTx = -1.0f;
-		double sumTs = 0.0;
-		// The reference ranks the top 4 and skips sot / solm / not at most 3 times (whisper.cpp:1945-1953); those are the only three
-		// banned ids, so the pick is simply the arg-max over every other eligible token.  Eligibility depends on the timestamp test
-		// below, hence two candidates from the same pass: the best text token and the best timestamp token.
-		Top1 bestTs = { -INFINITY, 0x7fffffff, 0 };
-		Top1 bestTx = { -INFINITY, 0x7fffffff, 0 };
-		for( int i = tid; i < nv; i += SM_THREADS )
-		{
-			const float p = pr[ i ] * inv;
-			if( a.rowInSmem ) gpr[ i ] = p; else pr[ i ] = p;
-			if( i < beg )
-			{
-				maxTx = fmaxf( maxTx, p );
-				if( i != a.tokenSot && i != a.tokenSolm && i != a.tokenNot ) bestTx = better( bestTx, Top1{ p, i, 0 } );
-			}
-			else if( i < tsEnd )
-			{
-				sumTs += (double)p;
-				bestTs = better( bestTs, Top1{ p, i, 0 } );
-			}
-		}
-		maxTx = blockMaxF( maxTx, sf );
-		sumTs = blockSumD( sumTs, sd );
-		bestTs = blockArgmax( bestTs, st );
-		bestTx = blockArgmax( bestTx, st );
-		const bool maskText = ( sumTs > (double)maxTx ) || forceTs;
-		__shared__ TieShared tieSh;
-		Top1 pick = bestTs;
-		if( !maskText ) pick = better( bestTx, bestTs );
-		if( pick.i == 0x7fffffff ) pick = Top1{ 0.0f, 0, 1 };
-		__syncthreads();     // the whole probability row is in global memory
-		pick = resolveTies( pick, a, b, maskText, isInitial, tieSh );
-		if( tid == 0 )
-		{
-			TokenData td;
-			td.id = pick.i;
-			td.tid = bestTs.i == 0x7fffffff ? 0 : bestTs.i;
-			td.p = pick.v;
-			td.pt = (float)( (double)bestTs.v / ( sumTs + 1e-10 ) );
-			td.ptsum = (float)sumTs;
-			a.out[ b ] = td;
-			if( a.nextTokens ) a.nextTokens[ b ] = td.id;
-			if( a.history && a.dStep && *a.dStep < a.histCap ) a.history[ (size_t)b * a.histCap + *a.dStep ] = td.id;
-		}
-	}
-
-	// The same sampler with one vocabulary row spread over a cluster of SC_CL CTAs: every CTA keeps its slice of the row in shared
-	// memory, the three row-wide reductions go through distributed shared memory (each CTA publishes its partial, cluster barrier,
-	// everybody combines the SC_CL partials in rank order).  8 rows on 8 SMs leave the other SMs idle.
+	// One vocabulary row spread over a cluster of SC_CL CTAs: every CTA keeps its slice of the row in shared memory, the three
+	// row-wide reductions go through distributed shared memory (each CTA publishes its partial, cluster barrier, everybody combines
+	// the SC_CL partials in rank order).  One CTA per row would leave most SMs idle and keep only a short row in shared memory.
 	struct ClusterPart
 	{
 		float mx, maxTx;
@@ -1088,47 +920,24 @@ namespace kern
 
 	cudaError_t sampleGreedy( const SampleArgs& a, cudaStream_t s )
 	{
-		SampleArgs sa = a;
-		// cluster size: 4 by default; WSP_SAMPLER_CLUSTER=0|4|8 for A/B runs
-		static const int clusterSize = []() { const char* e = getenv( "WSP_SAMPLER_CLUSTER" ); return e ? atoi( e ) : 4; }();
-		if( ( clusterSize == 4 || clusterSize == 8 ) && a.nVocab >= 4096 )
-		{
-			const int cl = clusterSize;
-			const size_t sliceBytes = (size_t)( ( a.nVocab + cl - 1 ) / cl ) * sizeof( float );
-			static PerDeviceMax sliceAttr;
-			{
-				const int nv = a.nVocab;
-				cudaError_t ea = sliceAttr.raise( (size_t)( ( nv + 3 ) / 4 ) * sizeof( float ), [ nv ]( size_t n4 ) {
-					cudaError_t e4 = cudaFuncSetAttribute( sample_cluster_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)n4 );
-					if( e4 != cudaSuccess ) return e4;
-					return cudaFuncSetAttribute( sample_cluster_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)( (size_t)( ( nv + 7 ) / 8 ) * sizeof( float ) ) );
-				} );
-				if( ea != cudaSuccess ) return ea;
-			}
-			cudaLaunchConfig_t cfg{};
-			cfg.gridDim = dim3( cl, a.B );
-			cfg.blockDim = dim3( SM_THREADS );
-			cfg.dynamicSmemBytes = sliceBytes;
-			cfg.stream = s;
-			cudaLaunchAttribute at[ 1 ];
-			at[ 0 ].id = cudaLaunchAttributeClusterDimension;
-			at[ 0 ].val.clusterDim.x = cl; at[ 0 ].val.clusterDim.y = 1; at[ 0 ].val.clusterDim.z = 1;
-			cfg.attrs = at;
-			cfg.numAttrs = 1;
-			cudaError_t e = cl == 4 ? cudaLaunchKernelEx( &cfg, sample_cluster_kernel<4>, sa ) : cudaLaunchKernelEx( &cfg, sample_cluster_kernel<8>, sa );
-			if( e != cudaSuccess ) return e;
-			return launchPdl( advance_kernel, dim3( 1 ), dim3( 1 ), 0, s, a.dNPast, a.N, const_cast<int*>( a.dForceTs ), a.dStep );
-		}
-		const size_t rowBytes = (size_t)a.nVocab * sizeof( float );
-		static const bool forceGlobal = getenv( "WSP_SAMPLER_GLOBAL" ) != nullptr;   // A/B switch for measurements
-		sa.rowInSmem = ( rowBytes <= 220 * 1024 && !forceGlobal ) ? 1 : 0;
-		static PerDeviceMax rowAttr;
-		if( sa.rowInSmem )
-		{
-			cudaError_t ea = rowAttr.raise( rowBytes, []( size_t n ) { return cudaFuncSetAttribute( sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)n ); } );
-			if( ea != cudaSuccess ) return ea;
-		}
-		cudaError_t e = launchPdl( sample_kernel, dim3( a.B ), dim3( SM_THREADS ), sa.rowInSmem ? rowBytes : 0, s, sa );
+		// 4 CTAs per row; a CTA's slice must fit its 227 KB of shared memory, which bounds the vocabulary at about 230 K tokens
+		constexpr int CL = 4;
+		if( !a.tieScratch ) return cudaErrorInvalidValue;
+		const size_t sliceBytes = (size_t)( ( a.nVocab + CL - 1 ) / CL ) * sizeof( float );
+		static PerDeviceMax sliceAttr;
+		cudaError_t e = sliceAttr.raise( sliceBytes, []( size_t n ) { return cudaFuncSetAttribute( sample_cluster_kernel<CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)n ); } );
+		if( e != cudaSuccess ) return e;
+		cudaLaunchConfig_t cfg{};
+		cfg.gridDim = dim3( CL, a.B );
+		cfg.blockDim = dim3( SM_THREADS );
+		cfg.dynamicSmemBytes = sliceBytes;
+		cfg.stream = s;
+		cudaLaunchAttribute at[ 1 ];
+		at[ 0 ].id = cudaLaunchAttributeClusterDimension;
+		at[ 0 ].val.clusterDim.x = CL; at[ 0 ].val.clusterDim.y = 1; at[ 0 ].val.clusterDim.z = 1;
+		cfg.attrs = at;
+		cfg.numAttrs = 1;
+		e = cudaLaunchKernelEx( &cfg, sample_cluster_kernel<CL>, a );
 		if( e != cudaSuccess ) return e;
 		// step-global state is advanced by a separate 1-thread kernel so that no CTA of the sampler races with it
 		return launchPdl( advance_kernel, dim3( 1 ), dim3( 1 ), 0, s, a.dNPast, a.N, const_cast<int*>( a.dForceTs ), a.dStep );

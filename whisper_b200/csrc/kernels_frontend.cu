@@ -2,16 +2,9 @@
 #include "kernels.cuh"
 #include "ptx.cuh"
 #include <math.h>
-#include <stdlib.h>
 
 namespace kern
 {
-	bool pdlEnabled()
-	{
-		static const bool on = []() { const char* e = getenv( "WSP_PDL" ); return !( e && e[ 0 ] == '0' ); }();
-		return on;
-	}
-
 	// float <-> order-preserving int, for atomicMax on floats of any sign
 	__device__ __forceinline__ int orderedFromFloat( float f )
 	{
@@ -111,7 +104,7 @@ namespace kern
 			melRaw[ (size_t)tid * nLen + frame ] = v;
 		}
 		// block max -> one atomic
-		for( int o = 16; o > 0; o >>= 1 ) v = fmaxf( v, __shfl_xor_sync( 0xffffffffu, v, o ) );
+		v = ptx::warp_max( v );
 		if( ( tid & 31 ) == 0 ) smax[ tid >> 5 ] = v;
 		__syncthreads();
 		if( tid == 0 )
@@ -225,12 +218,6 @@ namespace kern
 	// the f16 rounding is the activation conversion the next mul_mat performs (ggml.c:4592-4603).
 	constexpr int LN_MAX_V4 = 10;   // d <= 1280
 
-	__device__ __forceinline__ float warpSum( float v )
-	{
-		for( int o = 16; o > 0; o >>= 1 ) v += __shfl_xor_sync( 0xffffffffu, v, o );
-		return v;
-	}
-
 	__global__ void __launch_bounds__( 256 )
 		layernorm_f16_kernel( const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta, __half* __restrict__ out, int rows, int d )
 	{
@@ -248,7 +235,7 @@ namespace kern
 				v[ i ] = xr[ i * 32 + lane ];
 				sum += v[ i ].x + v[ i ].y + v[ i ].z + v[ i ].w;
 			}
-		const float mean = warpSum( sum ) / (float)d;
+		const float mean = ptx::warp_sum( sum ) / (float)d;
 		float sq = 0.0f;
 #pragma unroll
 		for( int i = 0; i < LN_MAX_V4; i++ )
@@ -257,7 +244,7 @@ namespace kern
 				v[ i ].x -= mean; v[ i ].y -= mean; v[ i ].z -= mean; v[ i ].w -= mean;
 				sq += v[ i ].x * v[ i ].x + v[ i ].y * v[ i ].y + v[ i ].z * v[ i ].z + v[ i ].w * v[ i ].w;
 			}
-		const float rstd = 1.0f / sqrtf( warpSum( sq ) / (float)d + 1e-5f );
+		const float rstd = 1.0f / sqrtf( ptx::warp_sum( sq ) / (float)d + 1e-5f );
 		const float4* g4 = reinterpret_cast<const float4*>( gamma );
 		const float4* b4 = reinterpret_cast<const float4*>( beta );
 		uint2* o2 = reinterpret_cast<uint2*>( out + (size_t)row * d );

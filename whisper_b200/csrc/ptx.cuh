@@ -1,5 +1,6 @@
 // Thin inline-PTX layer for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / mma_async / commit / wait) and the
-// wgmma shared-memory descriptor.  Everything here is hand-written for H100; there is no other target.
+// wgmma shared-memory descriptor; the decoder's mma.sync, streaming loads, cp.async, %globaltimer and warp reductions.
+// Everything here is hand-written for H100; there is no other target.
 //
 // The descriptor bit layout follows the PTX ISA's "Matrix Descriptor Format" for wgmma — the layouts are hardware facts.
 #pragma once
@@ -153,6 +154,61 @@ namespace ptx
 	// and block until every kernel this one depends on has completed and flushed its writes.
 	__device__ __forceinline__ void pdl_launch_dependents() { asm volatile( "griddepcontrol.launch_dependents;" ::: "memory" ); }
 	__device__ __forceinline__ void pdl_wait() { asm volatile( "griddepcontrol.wait;" ::: "memory" ); }
+
+	// ---------------------------------------------------------------------------------------------
+	// Decoder building blocks
+	//
+	// Butterfly reductions over the 32 lanes of a warp (xor 16, 8, 4, 2, 1): every lane ends with the same value, and the order of
+	// the additions is fixed, so results are bit-reproducible.
+	template<class T>
+	__device__ __forceinline__ T warp_sum( T v )
+	{
+		for( int o = 16; o > 0; o >>= 1 ) v += __shfl_xor_sync( 0xffffffffu, v, o );
+		return v;
+	}
+	__device__ __forceinline__ float warp_max( float v )
+	{
+		for( int o = 16; o > 0; o >>= 1 ) v = fmaxf( v, __shfl_xor_sync( 0xffffffffu, v, o ) );
+		return v;
+	}
+
+	// D += A * B, mma.sync m16n8k16 with f16 inputs and f32 accumulators: A fragment {a0, a1, a2, a3}, B fragment {b0, b1}
+	__device__ __forceinline__ void mma_m16n8k16( float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1 )
+	{
+		asm volatile(
+			"mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+			: "+f"( c[ 0 ] ), "+f"( c[ 1 ] ), "+f"( c[ 2 ] ), "+f"( c[ 3 ] )
+			: "r"( a0 ), "r"( a1 ), "r"( a2 ), "r"( a3 ), "r"( b0 ), "r"( b1 ) );
+	}
+	// the same with rows 8..15 of A zero (registers a1, a3): a unit of 8 weight rows
+	__device__ __forceinline__ void mma_m16n8k16_rows8( float* c, uint32_t a0, uint32_t a2, uint32_t b0, uint32_t b1 )
+	{
+		mma_m16n8k16( c, a0, 0u, a2, 0u, b0, b1 );
+	}
+
+	// 16-byte load of read-only data that is used once (weights): non-coherent path, not kept in L1
+	__device__ __forceinline__ uint4 ldg_stream( const uint4* p )
+	{
+		uint4 r;
+		asm volatile( "ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"( r.x ), "=r"( r.y ), "=r"( r.z ), "=r"( r.w ) : "l"( p ) );
+		return r;
+	}
+
+	// 16-byte asynchronous copy global -> shared (bypassing L1), its commit and the wait for every committed group
+	__device__ __forceinline__ void cp_async16( void* smemDst, const void* gmemSrc )
+	{
+		asm volatile( "cp.async.cg.shared.global [%0], [%1], 16;" ::"r"( smem_u32( smemDst ) ), "l"( gmemSrc ) : "memory" );
+	}
+	__device__ __forceinline__ void cp_async_commit() { asm volatile( "cp.async.commit_group;" ::: "memory" ); }
+	__device__ __forceinline__ void cp_async_wait_all() { asm volatile( "cp.async.wait_group 0;" ::: "memory" ); }
+
+	// nanoseconds of the global timer (debug marks, and the time limit of spin waits)
+	__device__ __forceinline__ unsigned long long globaltimer()
+	{
+		unsigned long long t;
+		asm volatile( "mov.u64 %0, %globaltimer;" : "=l"( t ) );
+		return t;
+	}
 
 	__device__ __forceinline__ float gelu_f16_semantics( float x )
 	{
