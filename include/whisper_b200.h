@@ -187,9 +187,20 @@ wsp_status wsp_timer_stop( wsp_context* c, float* ms );
  * around every launch.  kinds: 0 skinny GEMM, 1 cross-attention, 2 self-attention, 3 other (embedding, sampler) */
 wsp_status wsp_profile_decode( wsp_context* c, int32_t batch, int32_t n_steps, float ms_by_kind[ 4 ], int32_t launches_by_kind[ 4 ] );
 
-/* test hook: named intermediates as f32.  Names: "mel", "enc.conv1" ([2n][d] after GELU), "enc.x0" ([n][d] input of layer 0),
- * "enc.layers" (residual stream after the last layer), "encode-out" (ln_post, f16-rounded), "cross_k", "cross_v" ([L][T][d] of slot 0);
- * n = the audio positions of the last encode (1500 unless wsp_set_audio_ctx chose fewer). */
+/* test hook: named intermediates of chunk `slot`, as f32.  n = the audio positions of the last encode (1500 unless wsp_set_audio_ctx
+ * chose fewer), d = n_audio_state, H = n_audio_head, L = n_text_layer, Tp = 1536 (n_audio_ctx rounded up to 128).  The encoder
+ * tensors are those of the last encode; with wsp_debug_set_encoder_layers(k) the per-layer ones belong to layer k - 1.
+ *   "mel"                  [80][n_len]  log-mel of the slot
+ *   "enc.input"            [2n][80]     f16 mel window, frames [offset, offset + 2n), zero past n_len
+ *   "enc.conv1"            [2n][d]      f16 gelu(conv1 + bias)
+ *   "enc.x"                [n][d]       f32 residual stream: the input of layer k (all layers: the input of ln_post)
+ *   "enc.xn", "encode-out" [n][d]       f16 ln_post output
+ *   "enc.q", "enc.k"       [H][n][64]   f16 attention Q, K of the last encoded layer
+ *   "enc.vt"               [H][64][Tp]  f16 transposed V; columns [n, n rounded up to 128) are zero
+ *   "enc.attn"             [n][d]       f16 attention output (head h in columns [64h, 64h + 64))
+ *   "enc.h"                [n][4d]      f16 MLP hidden gelu(LN2(x) W1^T + b1) of the last encoded layer
+ *   "cross_k", "cross_v"   [L][H][n][64] f16 cross-attention memories (K scaled by 64^-0.25)
+ *   "dec.x"                [8][d]       f32 decoder residual stream (shared by all slots) */
 wsp_status wsp_get_tensor( wsp_context* c, const char* name, int32_t slot, float* dst, size_t cap_floats, size_t* n_floats );
 /* debug: run only the first n encoder layers (negative = all) */
 wsp_status wsp_debug_set_encoder_layers( wsp_context* c, int32_t n );

@@ -302,6 +302,7 @@ wsp_status wsp_get_tensor( wsp_context* cc, const char* name, int32_t slot, floa
 	else if( nm == "enc.q" ) { f16 = c.q + (size_t)slot * T * d; n = (size_t)T * d; }                                             // [H][T][64]
 	else if( nm == "enc.k" ) { f16 = c.k + (size_t)slot * T * d; n = (size_t)T * d; }
 	else if( nm == "enc.vt" ) { f16 = c.vt + (size_t)slot * H * 64 * c.Tp; n = (size_t)H * 64 * c.Tp; }                            // [H][64][Tp]
+	else if( nm == "enc.h" ) { f16 = c.h + (size_t)slot * T * 4 * d; n = (size_t)T * 4 * d; }                                     // [T][4d]
 	else if( nm == "cross_k" || nm == "cross_v" )
 	{
 		// gathered per layer below: [L][H][T][64] of this slot

@@ -27,37 +27,13 @@ namespace gemm
 		}
 	}
 
+	// f16 outputs (EPI_CONV1, EPI_QKV, EPI_BIAS_GELU_F16, EPI_CROSSKV)
 	template<int MODE>
 	__device__ __forceinline__ void epilogue( const EpiParams& ep, int m, int n0, float* v )
 	{
 		if( n0 >= ep.N )
 			return;
-		if constexpr( MODE == EPI_F32 )
-		{
-			if( m >= ep.M ) return;
-			float* dst = ep.out_f32 + (size_t)m * ep.ld + n0;
-			if( n0 + 32 <= ep.N && ( ep.ld & 3 ) == 0 )
-			{
-#pragma unroll
-				for( int i = 0; i < 8; i++ )
-				{
-					float4 o;
-					o.x = v[ i * 4 + 0 ]; o.y = v[ i * 4 + 1 ]; o.z = v[ i * 4 + 2 ]; o.w = v[ i * 4 + 3 ];
-					if( ep.bias )
-					{
-						const float4 b = *reinterpret_cast<const float4*>( ep.bias + n0 + i * 4 );
-						o.x += b.x; o.y += b.y; o.z += b.z; o.w += b.w;
-					}
-					reinterpret_cast<float4*>( dst )[ i ] = o;
-				}
-			}
-			else
-			{
-				for( int i = 0; i < 32 && n0 + i < ep.N; i++ )
-					dst[ i ] = v[ i ] + ( ep.bias ? ep.bias[ n0 + i ] : 0.0f );
-			}
-		}
-		else if constexpr( MODE == EPI_CONV1 )
+		if constexpr( MODE == EPI_CONV1 )
 		{
 			const int b = m / ep.rows_per_chunk;
 			const int t = m - b * ep.rows_per_chunk;
@@ -78,25 +54,6 @@ namespace gemm
 			for( int i = 0; i < 32; i++ )
 				v[ i ] = ptx::gelu_f16_semantics( v[ i ] + ep.bias[ n0 + i ] );
 			store_f16x32( ep.out_a + (size_t)( m + 1 ) * ep.ld + n0, v );
-		}
-		else if constexpr( MODE == EPI_CONV2 )
-		{
-			const int b = m / ep.rows_per_chunk;
-			const int j = m - b * ep.rows_per_chunk;
-			if( b >= ep.nchunks || j >= ep.valid_per_chunk ) return;
-			float* dst = ep.out_f32 + ( (size_t)b * ep.T + j ) * ep.ld + n0;
-			const float* pe = ep.pos + (size_t)j * ep.d + n0;
-#pragma unroll
-			for( int i = 0; i < 8; i++ )
-			{
-				const float4 p = *reinterpret_cast<const float4*>( pe + i * 4 );
-				float4 o;
-				o.x = ptx::gelu_f16_semantics( v[ i * 4 + 0 ] + ep.bias[ n0 + i * 4 + 0 ] ) + p.x;
-				o.y = ptx::gelu_f16_semantics( v[ i * 4 + 1 ] + ep.bias[ n0 + i * 4 + 1 ] ) + p.y;
-				o.z = ptx::gelu_f16_semantics( v[ i * 4 + 2 ] + ep.bias[ n0 + i * 4 + 2 ] ) + p.z;
-				o.w = ptx::gelu_f16_semantics( v[ i * 4 + 3 ] + ep.bias[ n0 + i * 4 + 3 ] ) + p.w;
-				reinterpret_cast<float4*>( dst )[ i ] = o;
-			}
 		}
 		else if constexpr( MODE == EPI_QKV )
 		{
@@ -130,23 +87,6 @@ namespace gemm
 					for( int i = 0; i < 32; i++ )
 						dst[ (size_t)i * ep.Tp + ( tz - t ) ] = __float2half_rn( 0.0f );
 				}
-			}
-		}
-		else if constexpr( MODE == EPI_BIAS_RESID )
-		{
-			if( m >= ep.M ) return;
-			const size_t off = (size_t)m * ep.ld + n0;
-#pragma unroll
-			for( int i = 0; i < 8; i++ )
-			{
-				const float4 b = *reinterpret_cast<const float4*>( ep.bias + n0 + i * 4 );
-				const float4 r = *reinterpret_cast<const float4*>( ep.resid + off + i * 4 );
-				float4 o;
-				o.x = v[ i * 4 + 0 ] + b.x + r.x;
-				o.y = v[ i * 4 + 1 ] + b.y + r.y;
-				o.z = v[ i * 4 + 2 ] + b.z + r.z;
-				o.w = v[ i * 4 + 3 ] + b.w + r.w;
-				*reinterpret_cast<float4*>( ep.out_f32 + off + i * 4 ) = o;
 			}
 		}
 		else if constexpr( MODE == EPI_BIAS_GELU_F16 )
@@ -193,7 +133,7 @@ namespace gemm
 	// each): half of every 32-byte sector is wasted and a 128-byte line needs 8 separate instructions.  For f32 outputs the
 	// 32 x 32 chunk is therefore read from the staging tile so that a thread owns one COLUMN: every load / store instruction of the
 	// warp then covers 32 consecutive elements of one output row.  `w` points at the thread's column in the staging tile
-	// (row stride STG_LD).
+	// (row stride STG_LD).  f32 outputs (EPI_F32, EPI_CONV2, EPI_BIAS_RESID).
 	template<int MODE>
 	__device__ __forceinline__ void epilogueT( const EpiParams& ep, int mBase, int n, const float* w )
 	{
@@ -206,21 +146,6 @@ namespace gemm
 			{
 				const int m = mBase + rr;
 				if( m < ep.M ) ep.out_f32[ (size_t)m * ep.ld + n ] = w[ rr * STG_LD ] + b;
-			}
-		}
-		else if constexpr( MODE == EPI_CONV1 )
-		{
-			const float b = ep.bias[ n ];
-			int cb = mBase / ep.rows_per_chunk;
-			int t = mBase - cb * ep.rows_per_chunk;
-#pragma unroll
-			for( int rr = 0; rr < 32; rr++ )
-			{
-				if( cb < ep.nchunks && t < ep.valid_per_chunk )
-					ep.out_a[ (size_t)( mBase + rr + 1 ) * ep.ld + n ] = __float2half_rn( ptx::gelu_f16_semantics( w[ rr * STG_LD ] + b ) );
-				else if( cb < ep.nchunks && mBase + rr + 1 < ep.nchunks * ep.rows_per_chunk )
-					ep.out_a[ (size_t)( mBase + rr + 1 ) * ep.ld + n ] = __float2half_rn( 0.0f );   // halo rows, as in epilogue<EPI_CONV1>
-				if( ++t == ep.rows_per_chunk ) { t = 0; cb++; }
 			}
 		}
 		else if constexpr( MODE == EPI_CONV2 )
@@ -253,24 +178,6 @@ namespace gemm
 				}
 			}
 		}
-		else if constexpr( MODE == EPI_QKV )
-		{
-			// Q and K only (the V^T part keeps the row-per-thread layout, which is the coalesced one for a transposed store)
-			const int which = n / ep.d;
-			const int nn = n - which * ep.d;
-			const int h = nn >> 6, e = nn & 63;
-			const float b = ep.bias[ n ];
-			__half* base = which == 0 ? ep.out_a : ep.out_b;
-			int cb = mBase / ep.T;
-			int t = mBase - cb * ep.T;
-#pragma unroll
-			for( int rr = 0; rr < 32; rr++ )
-			{
-				if( mBase + rr < ep.M )
-					base[ ( ( (size_t)cb * ep.H + h ) * ep.T + t ) * 64 + e ] = __float2half_rn( w[ rr * STG_LD ] + b );
-				if( ++t == ep.T ) { t = 0; cb++; }
-			}
-		}
 		else if constexpr( MODE == EPI_BIAS_RESID )
 		{
 			// the residual column 16 rows at a time ahead of the stores: issued one by one behind each store, its L2 round trips and
@@ -292,37 +199,6 @@ namespace gemm
 					const int m = mBase + h + rr;
 					if( m < ep.M ) ep.out_f32[ (size_t)m * ep.ld + n ] = w[ ( h + rr ) * STG_LD ] + b + rs[ rr ];
 				}
-			}
-		}
-		else if constexpr( MODE == EPI_BIAS_GELU_F16 )
-		{
-			const float b = ep.bias[ n ];
-#pragma unroll
-			for( int rr = 0; rr < 32; rr++ )
-			{
-				const int m = mBase + rr;
-				if( m < ep.M ) ep.out_a[ (size_t)m * ep.ld + n ] = __float2half_rn( ptx::gelu_f16_semantics( w[ rr * STG_LD ] + b ) );
-			}
-		}
-		else if constexpr( MODE == EPI_CROSSKV )
-		{
-			const int d2 = 2 * ep.d;
-			const int l = n / d2;
-			const int r = n - l * d2;
-			const bool isV = r >= ep.d;
-			const int nn = isV ? r - ep.d : r;
-			const int h = nn >> 6, e = nn & 63;
-			const float b = isV ? ep.bias[ n ] : 0.0f;
-			const float sc = isV ? 1.0f : ep.scale;
-			__half* base = ( isV ? ep.out_b : ep.out_a ) + (size_t)l * ep.layer_stride;
-			int cb = mBase / ep.T;
-			int t = mBase - cb * ep.T;
-#pragma unroll
-			for( int rr = 0; rr < 32; rr++ )
-			{
-				if( mBase + rr < ep.M )
-					base[ ( ( (size_t)cb * ep.H + h ) * ep.T + t ) * 64 + e ] = __float2half_rn( w[ rr * STG_LD ] * sc + b );
-				if( ++t == ep.T ) { t = 0; cb++; }
 			}
 		}
 	}

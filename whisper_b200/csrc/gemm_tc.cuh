@@ -24,7 +24,7 @@ namespace gemm
 
 	enum EpiMode : int
 	{
-		EPI_F32 = 0,          // out_f32[m][n] = acc (+ bias[n])                                  (tests, decoder prompt)
+		EPI_F32 = 0,          // out_f32[m][n] = acc (+ bias[n])                                  (the wsp_test_gemm hook only)
 		EPI_CONV1 = 1,        // f16 out[(m+1)][n] = gelu(acc + bias[n]), rows of padded time axis, halos zeroed (a3)
 		EPI_CONV2 = 2,        // f32 out[b*T+j][n] = gelu(acc + bias[n]) + pos[j][n]                (a4)
 		EPI_QKV = 3,          // Q,K head-major f16, V transposed f16                               (a6, a7)
