@@ -206,8 +206,8 @@ wsp_status wsp_get_tensor( wsp_context* c, const char* name, int32_t slot, float
 wsp_status wsp_debug_set_encoder_layers( wsp_context* c, int32_t n );
 /* The CPU reference accumulates the decoder's V^T*P product in f16, per thread (Whisper/source/ggml.c:4680-4722), so its logits
  * depend on its thread count.  n = the cpuThreads the reference would be run with (sFullParams::cpuThreads; default 4 =
- * whisper_full_default_params, Whisper/source/whisper.cpp:2605); the decoder reproduces that arithmetic for n = 1..16 (the
- * single-launch step kernel covers all of them; WSP_E_INVALIDARG above 16).  n = 0: plain f32 accumulation (per-op kernels). */
+ * whisper_full_default_params, Whisper/source/whisper.cpp:2605); the decoder reproduces that arithmetic for n = 1..16 in every
+ * step mode.  Any other n returns WSP_E_INVALIDARG. */
 wsp_status wsp_set_reference_threads( wsp_context* c, int32_t n );
 /* debug: 0 = launch the N = 1 decoder step kernel by kernel instead of replaying the captured CUDA graph */
 wsp_status wsp_debug_set_graph( wsp_context* c, int32_t on );

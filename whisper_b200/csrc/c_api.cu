@@ -1,5 +1,6 @@
 // extern "C" surface (include/whisper_b200.h) + kernel-level test hooks.
 #include "engine.h"
+#include "ref_arith.cuh"
 #include <algorithm>
 #include <math.h>
 #include <math.h>
@@ -378,7 +379,7 @@ wsp_status wsp_debug_set_encoder_layers( wsp_context* c, int32_t n )
 wsp_status wsp_set_reference_threads( wsp_context* c, int32_t n )
 {
 	if( !c ) return fail( WSP_E_POINTER, "context" );
-	if( n < 0 || n > 16 ) return fail( WSP_E_INVALIDARG, "reference thread count must be in [0, 16]" );
+	if( n < 1 || n > kern::kMaxRefThreads ) return fail( WSP_E_INVALIDARG, "reference thread count must be in [1, 16]" );
 	if( n != c->c->refThreads && c->c->stepGraph ) { cudaGraphExecDestroy( c->c->stepGraph ); c->c->stepGraph = nullptr; }
 	c->c->refThreads = n;
 	return WSP_OK;

@@ -31,9 +31,9 @@ namespace kern
 		constexpr int FL_WARPS = 8;                    // consumer warps
 		constexpr int FL_CONSUMERS = FL_WARPS * 32;
 		constexpr int FL_THREADS = FL_CONSUMERS + 32;  // + the producer warp
+		static_assert( FL_CONSUMERS == kAttnThreads, "softmaxRow (ref_arith.cuh) runs on the consumer warps" );
 		constexpr int FL_NSMAX = 32;
 		constexpr int FL_MAXT = 1536;
-		constexpr int FL_MAXPARTS = 16;                // reference thread counts whose V^T*P split the kernel reproduces
 		constexpr int FL_SMEM_MAX = 232448;            // 227 KB opt-in limit per CTA on sm_90
 		constexpr uint32_t SENT32 = 0xFFFFFFFFu;
 
@@ -61,7 +61,7 @@ namespace kern
 			l.sp = o; o += FL_MAXT * 4;
 			l.bias = o; o += 256 * 4;
 			l.xres = o; o += 16 * 16 * 4;
-			l.so = o; o += FL_MAXPARTS * 64 * 4;
+			l.so = o; o += kMaxRefThreads * 64 * 4;
 			l.sred = o; o += 64;
 			l.qkv = o; o += 3 * 128;
 			l.bars = o; o += 2 * FL_NSMAX * 8;
@@ -253,31 +253,6 @@ namespace kern
 				}
 			}
 			return lmax;
-		}
-
-		// softmax over sp[0, n) exactly as the reference does it: max in f32, e = f16-table exp, sum, scale by 1/sum (ggml.c:5026-5095)
-		__device__ __forceinline__ void softmaxRow( float* sp, int n, float lmax, float* sred, int tid, int warp, int lane )
-		{
-			lmax = ptx::warp_max( lmax );
-			if( lane == 0 ) sred[ warp ] = lmax;
-			consumerSync();
-			float mx = sred[ 0 ];
-			for( int w = 1; w < FL_WARPS; w++ ) mx = fmaxf( mx, sred[ w ] );
-			float lsum = 0.0f;
-			for( int j = tid; j < n; j += FL_CONSUMERS )
-			{
-				const float e = expF16Table( sp[ j ] - mx );
-				sp[ j ] = e;
-				lsum += e;
-			}
-			lsum = ptx::warp_sum( lsum );
-			if( lane == 0 ) sred[ FL_WARPS + warp ] = lsum;   // (the maxima in sred[0..8) may still be being read)
-			consumerSync();
-			float tot = 0.0f;
-			for( int w = 0; w < FL_WARPS; w++ ) tot += sred[ FL_WARPS + w ];
-			const float inv = 1.0f / tot;
-			for( int j = tid; j < n; j += FL_CONSUMERS ) sp[ j ] *= inv;
-			consumerSync();
 		}
 
 		// one f32 row of D elements from an exchange buffer: every lane polls its N4 16-byte pieces until no sentinel is left
@@ -542,7 +517,7 @@ namespace kern
 			int nPast = *a.dNPast;              // read once: the sampler advances it after this launch
 			nPast = max( 0, min( nPast, a.nTextCtx - 1 ) );
 			const int nkvOld = nPast;           // rows of earlier tokens in the self-KV cache
-			const int parts = a.refThreads > 0 ? a.refThreads : 4;
+			const int parts = a.refThreads;
 			const size_t colsD = (size_t)a.maxB * D;
 			const size_t exLayer = colsD * 32;
 			const FlowGeom& g = a.g;
@@ -822,7 +797,7 @@ namespace kern
 							}
 							if( self ) lmax = scoreRows<1>( sqkv + 128, 1, nOld, qf, sp, warp, FL_WARPS, lane, lmax );   // this step's own K row
 							sub( 2 );
-							softmaxRow( sp, n, lmax, sred, tid, warp, lane );
+							softmaxRow<consumerSync>( sp, n, lmax, sred, tid, warp, lane );
 							sub( 3 );
 							{
 								const int q = tid >> 6, e = tid & 63;
@@ -1193,7 +1168,7 @@ namespace kern
 	bool flowSupported( int d, int B, int T, int H, int nTextCtx, int refThreads, int grid )
 	{
 		if( B < 1 || B > 16 || T > FL_MAXT || T < 1 || H * 64 != d || nTextCtx > FL_MAXT ) return false;
-		if( refThreads < 1 || refThreads > FL_MAXPARTS ) return false;   // 0 (plain f32 accumulation, not the reference's arithmetic) runs on the per-op path
+		if( refThreads < 1 || refThreads > kMaxRefThreads ) return false;
 		if( !( d == 128 || d == 384 || d == 512 || d == 768 || d == 1024 || d == 1280 ) ) return false;
 		const FlowGeom g = flowGeometry( d, 51865, grid );
 		if( g.R1 > 16 || g.slabFloats > 256 ) return false;

@@ -21,6 +21,7 @@ namespace kern
 	{
 		constexpr int MG_THREADS = 256;
 		constexpr int MG_WARPS = 8;
+		static_assert( MG_THREADS == kAttnThreads, "the attention phases use the 256-thread helpers of ref_arith.cuh" );
 		constexpr int MG_PAD = 32;         // halves of padding per activation row (conflict-free LDS.128)
 		constexpr int MG_ROWS = 8;         // weight rows per unit
 		constexpr int MG_MAXUPB = 4;       // units per register batch
@@ -447,49 +448,8 @@ namespace kern
 					sm.sp[ j ] = s;
 					lmax = fmaxf( lmax, s );
 				}
-				lmax = ptx::warp_max( lmax );
-				if( lane == 0 ) sred[ warp ] = lmax;
-				__syncthreads();
-				float mx = sred[ 0 ];
-				for( int w = 1; w < MG_WARPS; w++ ) mx = fmaxf( mx, sred[ w ] );
-				__syncthreads();
-				float lsum = 0.0f;
-				for( int j = tid; j < nkv; j += MG_THREADS )
-				{
-					const float e = expF16Table( sm.sp[ j ] - mx );
-					sm.sp[ j ] = e;
-					lsum += e;
-				}
-				lsum = ptx::warp_sum( lsum );
-				if( lane == 0 ) sred[ warp ] = lsum;
-				__syncthreads();
-				float tot = 0.0f;
-				for( int w = 0; w < MG_WARPS; w++ ) tot += sred[ w ];
-				const float inv = 1.0f / tot;
-				for( int j = tid; j < nkv; j += MG_THREADS ) sm.sp[ j ] *= inv;
-				__syncthreads();
-				const int parts = a.refThreads > 0 ? a.refThreads : 4;
-				const int dc = ( nkv + parts - 1 ) / parts;
-				for( int idx = tid; idx < parts * 64; idx += MG_THREADS )
-				{
-					const int part = idx >> 6, e = idx & 63;
-					const int j0 = min( part * dc, nkv ), j1 = min( ( part + 1 ) * dc, nkv );
-					float y;
-					if( a.refThreads > 0 ) y = pvChainF16( sm.sp, sV + e, 64, j0, j1 );
-					else
-					{
-						y = 0.0f;
-						for( int j = j0; j < j1; j++ ) y += sm.sp[ j ] * __half2float( sV[ (size_t)j * 64 + e ] );
-					}
-					so[ idx ] = y;
-				}
-				__syncthreads();
-				if( tid < 64 )
-				{
-					float acc = so[ tid ];
-					for( int k = 1; k < parts; k++ ) acc += so[ k * 64 + tid ];
-					a.attn[ (size_t)b * d + h * 64 + tid ] = __float2half_rn( acc );
-				}
+				softmaxRow<ctaSync>( sm.sp, nkv, lmax, sred, tid, warp, lane );
+				pvSplitF16( sm.sp, sV, nkv, a.refThreads, ( nkv + a.refThreads - 1 ) / a.refThreads, so, a.attn + (size_t)b * d + h * 64, tid );
 				__syncthreads();
 			}
 		}
@@ -497,10 +457,9 @@ namespace kern
 		// -----------------------------------------------------------------------------------------------------------
 		// cross attention over the encoder's f16 K/V memories: units = (chunk, head).  The V tile and the first batch of K rows are
 		// requested BEFORE the grid barrier (they do not depend on this step), q is read after it.
-		constexpr int CA_U = 12;
 		struct CrossPrefetch
 		{
-			uint4 u[ CA_U ];
+			uint4 u[ kKBatch ];
 			int unit;
 		};
 		__device__ __forceinline__ void crossPrefetch( const MegaArgs& a, const MegaLayer& L, CrossPrefetch& pf, const Smem& sm, int unit, int warp, int lane, int tid )
@@ -508,121 +467,34 @@ namespace kern
 			pf.unit = unit;
 			if( unit >= a.B * a.H ) return;
 			const int T = a.T;
-			const int b = unit / a.H, h = unit - b * a.H;
-			const size_t base = ( (size_t)b * a.H + h ) * T * 64;
+			const size_t base = (size_t)unit * T * 64;   // unit = b * H + h
 			const uint4* V4 = reinterpret_cast<const uint4*>( L.crossV + base );
-			const uint4* K4 = reinterpret_cast<const uint4*>( L.crossK + base );
 			uint4* sv = reinterpret_cast<uint4*>( sm.a );
 			for( int idx = tid; idx < T * 8; idx += MG_THREADS ) ptx::cp_async16( sv + idx, V4 + idx );
 			ptx::cp_async_commit();
-			const int sub = lane & 7, rgrp = lane >> 3;
-			const int jb = warp * 4 + rgrp;
-#pragma unroll
-			for( int k = 0; k < CA_U; k++ )
-			{
-				const int j = jb + k * MG_WARPS * 4;
-				pf.u[ k ] = j < T ? K4[ (size_t)j * 8 + sub ] : make_uint4( 0, 0, 0, 0 );
-			}
+			kStreamPrefetch( pf.u, reinterpret_cast<const uint4*>( L.crossK + base ), T, warp, lane );
 		}
 		__device__ void crossAttnPhase( const MegaArgs& a, const MegaLayer& L, int d, CrossPrefetch& pf, const Smem& sm, int warp, int lane, int tid )
 		{
 			const int T = a.T, H = a.H;
 			float* sred = sm.misc + 64;
 			float* so = sm.red;
-			const int sub = lane & 7, rgrp = lane >> 3;
-			constexpr int JSTEP = MG_WARPS * 4;
 			bool first = true;
 			for( int unit = blockIdx.x; unit < a.B * H; unit += gridDim.x )
 			{
 				if( !first ) { crossPrefetch( a, L, pf, sm, unit, warp, lane, tid ); }
 				first = false;
 				const int b = unit / H, h = unit - b * H;
-				const size_t base = ( (size_t)b * H + h ) * T * 64;
-				const uint4* K4 = reinterpret_cast<const uint4*>( L.crossK + base );
+				const uint4* K4 = reinterpret_cast<const uint4*>( L.crossK + (size_t)unit * T * 64 );
 				float qf[ 8 ];
 #pragma unroll
-				for( int e = 0; e < 8; e++ ) qf[ e ] = __half2float( __float2half_rn( __ldcg( a.q + (size_t)b * d + h * 64 + sub * 8 + e ) ) );
-				float lmax = -INFINITY;
-				int jb = warp * 4 + rgrp;
-				while( jb < T )
-				{
-#pragma unroll
-					for( int k = 0; k < CA_U; k++ )
-					{
-						const int j = jb + k * JSTEP;
-						const __half2* h2 = reinterpret_cast<const __half2*>( &pf.u[ k ] );
-						float s = 0.0f;
-#pragma unroll
-						for( int e = 0; e < 4; e++ )
-						{
-							const float2 f = __half22float2( h2[ e ] );
-							s += f.x * qf[ e * 2 ] + f.y * qf[ e * 2 + 1 ];
-						}
-						s += __shfl_xor_sync( 0xffffffffu, s, 1 );
-						s += __shfl_xor_sync( 0xffffffffu, s, 2 );
-						s += __shfl_xor_sync( 0xffffffffu, s, 4 );
-						if( j < T )
-						{
-							if( sub == 0 ) sm.sp[ j ] = s;
-							lmax = fmaxf( lmax, s );
-						}
-					}
-					jb += JSTEP * CA_U;
-					if( jb < T )
-					{
-#pragma unroll
-						for( int k = 0; k < CA_U; k++ )
-						{
-							const int j = jb + k * JSTEP;
-							pf.u[ k ] = j < T ? K4[ (size_t)j * 8 + sub ] : make_uint4( 0, 0, 0, 0 );
-						}
-					}
-				}
-				lmax = ptx::warp_max( lmax );
-				if( lane == 0 ) sred[ warp ] = lmax;
-				__syncthreads();
-				float mx = sred[ 0 ];
-				for( int w = 1; w < MG_WARPS; w++ ) mx = fmaxf( mx, sred[ w ] );
-				__syncthreads();
-				float lsum = 0.0f;
-				for( int j = tid; j < T; j += MG_THREADS )
-				{
-					const float e = expF16Table( sm.sp[ j ] - mx );
-					sm.sp[ j ] = e;
-					lsum += e;
-				}
-				lsum = ptx::warp_sum( lsum );
-				if( lane == 0 ) sred[ warp ] = lsum;
-				__syncthreads();
-				float tot = 0.0f;
-				for( int w = 0; w < MG_WARPS; w++ ) tot += sred[ w ];
-				const float inv = 1.0f / tot;
-				for( int j = tid; j < T; j += MG_THREADS ) sm.sp[ j ] *= inv;
+				for( int e = 0; e < 8; e++ ) qf[ e ] = __half2float( __float2half_rn( __ldcg( a.q + (size_t)b * d + h * 64 + ( lane & 7 ) * 8 + e ) ) );
+				const float lmax = kStreamScores( pf.u, K4, T, qf, sm.sp, warp, lane );
+				softmaxRow<ctaSync>( sm.sp, T, lmax, sred, tid, warp, lane );
 				ptx::cp_async_wait_all();
 				__syncthreads();
-				const __half* sv = reinterpret_cast<const __half*>( sm.a );
-				const int parts = a.refThreads > 0 ? a.refThreads : 4;
-				const int dc = ( T + parts - 1 ) / parts;
-				for( int idx = tid; idx < parts * 64; idx += MG_THREADS )
-				{
-					const int part = idx >> 6, e = idx & 63;
-					const int j0 = min( part * dc, T ), j1 = min( ( part + 1 ) * dc, T );
-					float y;
-					if( a.refThreads > 0 ) y = pvChainF16( sm.sp, sv + e, 64, j0, j1 );
-					else
-					{
-						y = 0.0f;
-						for( int j = j0; j < j1; j++ ) y += sm.sp[ j ] * __half2float( sv[ (size_t)j * 64 + e ] );
-					}
-					so[ idx ] = y;
-				}
-				__syncthreads();
-				if( tid < 64 )
-				{
-					float acc = so[ tid ];
-					for( int k = 1; k < parts; k++ ) acc += so[ k * 64 + tid ];
-					a.attn[ (size_t)b * d + h * 64 + tid ] = __float2half_rn( acc );
-				}
+				pvSplitF16( sm.sp, reinterpret_cast<const __half*>( sm.a ), T, a.refThreads, ( T + a.refThreads - 1 ) / a.refThreads, so,
+					a.attn + (size_t)b * d + h * 64, tid );
 				__syncthreads();
 			}
 		}

@@ -154,7 +154,7 @@ namespace wsp
 		int lastLogitRows = 0;
 		int nPastHost = 0;              // host mirror of the device-resident n_past (it advances on the device between graph replays)
 		int debugEncLayers = -1;
-		int refThreads = 4;             // reference CPU thread count whose V^T*P arithmetic the decoder reproduces (0 = exact)
+		int refThreads = 4;             // reference CPU thread count whose V^T*P arithmetic the decoder reproduces (1..16)
 
 		// tensor maps (built once; M of a launch limits the rows touched)
 		CUtensorMap mapMel, mapConv1Even, mapConv1Odd, mapXn, mapAttn, mapH;

@@ -95,7 +95,7 @@ namespace kern
 	};
 	cudaError_t skinnyGemm( const SkinnyArgs& a, cudaStream_t s );
 
-	// refThreads: reproduce the reference's f16-accumulated V^T*P for that many CPU threads (see kernels_decode.cu); 0 = exact f32
+	// refThreads (1..kMaxRefThreads): reproduce the reference's f16-accumulated V^T*P for that many CPU threads (ref_arith.cuh)
 	// self attention over the f16 self-KV cache, causal: query i of chunk b sees keys [0, nPast+i]   (a14)
 	cudaError_t selfAttnDecode( const float* q, const __half* kCache, const __half* vCache, __half* out, int B, int N, int H, int d, int nTextCtx, const int* dNPast, int refThreads, cudaStream_t s );
 	// cross attention over the f16 cross-KV memory [b][h][T][64]                                       (a15)

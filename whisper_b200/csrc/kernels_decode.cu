@@ -237,10 +237,10 @@ namespace kern
 
 	static size_t skinnySmem( int K ) { return (size_t)SK_COLS * ( K + SK_PAD ) * sizeof( __half ) + (size_t)SK_WARPS * SK_ROWS * SK_COLS * sizeof( float ); }
 	static PerDeviceMax g_skinnyAttr;
-	static cudaError_t crossPrepare( int T );
+	static cudaError_t attnPrepare();
 	cudaError_t prepare( int maxK )
 	{
-		cudaError_t ce = crossPrepare( 1500 );
+		cudaError_t ce = attnPrepare();
 		if( ce != cudaSuccess ) return ce;
 		return g_skinnyAttr.raise( skinnySmem( maxK ), []( size_t n ) { return cudaFuncSetAttribute( skinny_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)n ); } );
 	}
@@ -258,287 +258,83 @@ namespace kern
 	}
 
 	// ---------------------------------------------------------------------------------------------------------------
-	// V^T * P and the softmax exponential with the reference's arithmetic: pvChainF16 / expF16Table in ref_arith.cuh
-	constexpr int PV_MAX_THREADS = 16;
+	// Decoder attention, one CTA per (chunk, head, query): softmax( q . K ) . V over an f16 memory [b][h][rows][64], with the
+	// reference's arithmetic (ref_arith.cuh).
+	//   SELF:  the self-KV cache, rows = n_text_ctx.  Causal: query i of chunk b sees keys [0, nPast + i]; the reference cuts its
+	//          threads' key ranges from the keys of the whole call, min( nPast + N, n_text_ctx ).  Oracle: whisper.cpp:1616-1661 —
+	//          K*Q (Q rounded to f16 by the mul_mat, ggml.c:4599), causal mask, softmax, V^T * P.
+	//   cross: the encoder's cross-KV memory, rows = T, no mask.  Oracle: whisper.cpp:1688-1749 (K pre-scaled at encode time :1465).
+	//          Its 2*T*d bytes per layer are the dominant per-chunk HBM traffic of a decode step (SURVEY.md §8 a15).
+	// K streams through registers (kStreamScores, every access a coalesced 16-byte load); V streams into shared memory by cp.async
+	// behind the scoring.  The cross memory was written by the encoder before the PDL chain, so both are requested before the
+	// dependency wait; the self cache gets this call's rows from the preceding QKV GEMM, so nothing of it (nor n_past) is read before.
+	template<bool SELF>
+	constexpr int attnMaxRows = SELF ? 448 : 1500;
 
-	// ---------------------------------------------------------------------------------------------------------------
-	// Decoder self-attention, one CTA per (chunk, head, query).  Oracle: whisper.cpp:1616-1661 — K*Q (Q rounded to f16 by the
-	// mul_mat, ggml.c:4599), causal mask, softmax, V^T * P.  KV cache rows are head-major [b][h][pos][64] f16.
-	constexpr int SA_THREADS = 128;
-	constexpr int SA_MAXKV = 448;
-
-	__global__ void __launch_bounds__( SA_THREADS )
-		self_attn_decode_kernel( const float* __restrict__ q, const __half* __restrict__ kCache, const __half* __restrict__ vCache, __half* __restrict__ out,
-			int N, int H, int d, int nTextCtx, const int* __restrict__ dNPast, int refThreads )
+	template<bool SELF>
+	__global__ void __launch_bounds__( kAttnThreads )
+		attn_decode_kernel( const float* __restrict__ q, const __half* __restrict__ kMem, const __half* __restrict__ vMem, __half* __restrict__ out,
+			int N, int H, int d, int rows, const int* __restrict__ dNPast, int refThreads )
 	{
-		__shared__ float sq[ 64 ];
-		__shared__ float sp[ SA_MAXKV ];
-		__shared__ float sred[ SA_THREADS / 32 ];
-		__shared__ float so[ PV_MAX_THREADS ][ 64 ];
-		ptx::pdl_launch_dependents();
-		ptx::pdl_wait();
-		const int bh = blockIdx.x;
-		const int b = bh / H, h = bh - b * H;
-		const int i = blockIdx.y;
-		const int tid = threadIdx.x;
-		const int nkv = min( *dNPast + i + 1, nTextCtx );   // causal: keys visible to query i
-		const int nkvAll = min( *dNPast + N, nTextCtx );     // columns of the KQ matrix the reference partitions over its threads
-		const int col = b * N + i;
-		if( tid < 64 )
-			sq[ tid ] = __half2float( __float2half_rn( q[ (size_t)col * d + h * 64 + tid ] ) );
-		__syncthreads();
-		const __half* kb = kCache + ( (size_t)b * H + h ) * nTextCtx * 64;
-		const __half* vb = vCache + ( (size_t)b * H + h ) * nTextCtx * 64;
-		float lmax = -INFINITY;
-		for( int j = tid; j < nkv; j += SA_THREADS )
-		{
-			const uint4* kr = reinterpret_cast<const uint4*>( kb + (size_t)j * 64 );
-			float s = 0.0f;
-#pragma unroll
-			for( int c = 0; c < 8; c++ )
-			{
-				const uint4 u = kr[ c ];
-				const __half2* h2 = reinterpret_cast<const __half2*>( &u );
-#pragma unroll
-				for( int e = 0; e < 4; e++ )
-				{
-					const float2 f = __half22float2( h2[ e ] );
-					s += f.x * sq[ c * 8 + e * 2 ] + f.y * sq[ c * 8 + e * 2 + 1 ];
-				}
-			}
-			sp[ j ] = s;
-			lmax = fmaxf( lmax, s );
-		}
-		lmax = ptx::warp_max( lmax );
-		if( ( tid & 31 ) == 0 ) sred[ tid >> 5 ] = lmax;
-		__syncthreads();
-		float mx = sred[ 0 ];
-		for( int w = 1; w < SA_THREADS / 32; w++ ) mx = fmaxf( mx, sred[ w ] );
-		__syncthreads();
-		float lsum = 0.0f;
-		for( int j = tid; j < nkv; j += SA_THREADS )
-		{
-			const float e = expF16Table( sp[ j ] - mx );
-			sp[ j ] = e;
-			lsum += e;
-		}
-		lsum = ptx::warp_sum( lsum );
-		if( ( tid & 31 ) == 0 ) sred[ tid >> 5 ] = lsum;
-		__syncthreads();
-		float tot = 0.0f;
-		for( int w = 0; w < SA_THREADS / 32; w++ ) tot += sred[ w ];
-		const float inv = 1.0f / tot;
-		for( int j = tid; j < nkv; j += SA_THREADS ) sp[ j ] *= inv;   // the reference normalises P before V^T*P (ggml.c:5085-5090)
-		__syncthreads();
-		const int e = tid & 63;
-		if( refThreads > 0 )
-		{
-			// reference arithmetic: refThreads f16 chains over contiguous key ranges, summed in f32 in thread order
-			const int dc = ( nkvAll + refThreads - 1 ) / refThreads;
-			for( int part = tid >> 6; part < refThreads; part += SA_THREADS / 64 )
-			{
-				const int j0 = min( part * dc, nkv ), j1 = min( ( part + 1 ) * dc, nkv );   // masked keys contribute exactly 0
-				so[ part ][ e ] = pvChainF16( sp, vb + e, (size_t)64, j0, j1 );
-			}
-			__syncthreads();
-			if( tid < 64 )
-			{
-				float acc = so[ 0 ][ tid ];
-				for( int k = 1; k < refThreads; k++ ) acc += so[ k ][ tid ];
-				out[ (size_t)col * d + h * 64 + tid ] = __float2half_rn( acc );
-			}
-		}
-		else
-		{
-			const int half = tid >> 6;
-			float o = 0.0f;
-			for( int j = half; j < nkv; j += 2 )
-				o += sp[ j ] * __half2float( vb[ (size_t)j * 64 + e ] );
-			so[ half ][ e ] = o;
-			__syncthreads();
-			if( tid < 64 )
-				out[ (size_t)col * d + h * 64 + tid ] = __float2half_rn( so[ 0 ][ tid ] + so[ 1 ][ tid ] );
-		}
-	}
-	cudaError_t selfAttnDecode( const float* q, const __half* kCache, const __half* vCache, __half* out, int B, int N, int H, int d, int nTextCtx, const int* dNPast, int refThreads, cudaStream_t s )
-	{
-		if( nTextCtx > SA_MAXKV || refThreads < 0 || refThreads > PV_MAX_THREADS ) return cudaErrorInvalidValue;
-		dim3 grid( B * H, N );
-		return launchPdl( self_attn_decode_kernel, grid, dim3( SA_THREADS ), 0, s, q, kCache, vCache, out, N, H, d, nTextCtx, dNPast, refThreads );
-	}
-
-	// ---------------------------------------------------------------------------------------------------------------
-	// Decoder cross-attention, one CTA per (chunk, head, query); K and V memories are [b][h][T][64] f16, written by the
-	// encoder's cross-KV GEMM epilogue.  Oracle: whisper.cpp:1688-1749 (no mask, K pre-scaled at encode time :1465).
-	// The per-sequence 2*T*d bytes per layer are the dominant per-chunk HBM traffic of a decode step (SURVEY.md §8 a15):
-	// every access below is a 16-byte load, 8 lanes per 128-byte row, fully coalesced.
-	constexpr int CA_THREADS = 256;
-	constexpr int CA_MAXT = 1536;
-	constexpr int CA_UNROLL = 12;
-
-	__global__ void __launch_bounds__( CA_THREADS )
-		cross_attn_decode_kernel( const float* __restrict__ q, const __half* __restrict__ kMem, const __half* __restrict__ vMem, __half* __restrict__ out,
-			int N, int H, int d, int T, int refThreads )
-	{
-		extern __shared__ __align__( 16 ) uint8_t ca_smem[];   // the whole V tile of this (chunk, head): T x 128 bytes
-		__shared__ float sp[ CA_MAXT ];
-		__shared__ float sred[ CA_THREADS / 32 ];
-		__shared__ float so[ CA_THREADS / 32 ][ 4 ][ 64 ];   // per warp, per row-group partial outputs (8 KB) | [refThreads][64]
+		extern __shared__ __align__( 16 ) uint8_t at_smem[];   // the V rows of this (chunk, head): rows x 128 bytes
+		__shared__ float sp[ attnMaxRows<SELF> ];
+		__shared__ float sred[ 16 ];
+		__shared__ float so[ kMaxRefThreads * 64 ];
 		const int bh = blockIdx.x;
 		const int b = bh / H, h = bh - b * H;
 		const int i = blockIdx.y;
 		const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 		const int col = b * N + i;
-		const int sub = lane & 7;        // which 16-byte chunk of the 128-byte row
-		const int rgrp = lane >> 3;      // row within a group of 4
-		const uint4* K4 = reinterpret_cast<const uint4*>( kMem + (size_t)bh * T * 64 );
-		const uint4* V4 = reinterpret_cast<const uint4*>( vMem + (size_t)bh * T * 64 );
+		const uint4* K4 = reinterpret_cast<const uint4*>( kMem + (size_t)bh * rows * 64 );
+		const uint4* V4 = reinterpret_cast<const uint4*>( vMem + (size_t)bh * rows * 64 );
 
 		ptx::pdl_launch_dependents();
-		// V streams into shared memory (cp.async, no registers) behind the whole K phase.  Neither V nor K depends on the previous
-		// kernel (the cross-KV memories were written by the encoder), so both prefetches are issued before the dependency wait.
+		if( SELF ) ptx::pdl_wait();
+		const int nPast = SELF ? *dNPast : 0;
+		const int nkv = SELF ? min( nPast + i + 1, rows ) : rows;      // keys visible to query i
+		const int nkvAll = SELF ? min( nPast + N, rows ) : rows;     // keys the reference partitions over its threads
 		{
-			uint4* sv = reinterpret_cast<uint4*>( ca_smem );
-			for( int idx = tid; idx < T * 8; idx += CA_THREADS ) ptx::cp_async16( sv + idx, V4 + idx );
+			uint4* sv = reinterpret_cast<uint4*>( at_smem );
+			for( int idx = tid; idx < nkv * 8; idx += kAttnThreads ) ptx::cp_async16( sv + idx, V4 + idx );
 			ptx::cp_async_commit();
 		}
-		constexpr int JSTEP = ( CA_THREADS / 32 ) * 4;
-		int jb = warp * 4 + rgrp;
-		uint4 u[ CA_UNROLL ];
-#pragma unroll
-		for( int k = 0; k < CA_UNROLL; k++ )
-		{
-			const int j = jb + k * JSTEP;
-			u[ k ] = j < T ? K4[ (size_t)j * 8 + sub ] : make_uint4( 0, 0, 0, 0 );
-		}
+		uint4 u[ kKBatch ];
+		kStreamPrefetch( u, K4, nkv, warp, lane );
+		if( !SELF ) ptx::pdl_wait();
 
-		ptx::pdl_wait();
 		float qf[ 8 ];
 #pragma unroll
 		for( int e = 0; e < 8; e++ )
-			qf[ e ] = __half2float( __float2half_rn( q[ (size_t)col * d + h * 64 + sub * 8 + e ] ) );
-
-		// scores: a warp covers 4 key rows per load instruction (512 contiguous bytes), CA_UNROLL loads in flight per lane
-		float lmax = -INFINITY;
-		while( jb < T )
-		{
-#pragma unroll
-			for( int k = 0; k < CA_UNROLL; k++ )
-			{
-				const int j = jb + k * JSTEP;
-				const __half2* h2 = reinterpret_cast<const __half2*>( &u[ k ] );
-				float s = 0.0f;
-#pragma unroll
-				for( int e = 0; e < 4; e++ )
-				{
-					const float2 f = __half22float2( h2[ e ] );
-					s += f.x * qf[ e * 2 ] + f.y * qf[ e * 2 + 1 ];
-				}
-				s += __shfl_xor_sync( 0xffffffffu, s, 1 );
-				s += __shfl_xor_sync( 0xffffffffu, s, 2 );
-				s += __shfl_xor_sync( 0xffffffffu, s, 4 );
-				if( j < T )
-				{
-					if( sub == 0 ) sp[ j ] = s;
-					lmax = fmaxf( lmax, s );
-				}
-			}
-			jb += JSTEP * CA_UNROLL;
-			if( jb < T )
-			{
-#pragma unroll
-				for( int k = 0; k < CA_UNROLL; k++ )
-				{
-					const int j = jb + k * JSTEP;
-					u[ k ] = j < T ? K4[ (size_t)j * 8 + sub ] : make_uint4( 0, 0, 0, 0 );
-				}
-			}
-		}
-		lmax = ptx::warp_max( lmax );
-		if( lane == 0 ) sred[ warp ] = lmax;
-		__syncthreads();
-		float mx = sred[ 0 ];
-		for( int w = 1; w < CA_THREADS / 32; w++ ) mx = fmaxf( mx, sred[ w ] );
-		__syncthreads();
-		float lsum = 0.0f;
-		for( int j = tid; j < T; j += CA_THREADS )
-		{
-			const float e = expF16Table( sp[ j ] - mx );
-			sp[ j ] = e;
-			lsum += e;
-		}
-		lsum = ptx::warp_sum( lsum );
-		if( lane == 0 ) sred[ warp ] = lsum;
-		__syncthreads();
-		float tot = 0.0f;
-		for( int w = 0; w < CA_THREADS / 32; w++ ) tot += sred[ w ];
-		const float inv = 1.0f / tot;
-		for( int j = tid; j < T; j += CA_THREADS ) sp[ j ] *= inv;   // normalised P (ggml.c:5085-5090)
+			qf[ e ] = __half2float( __float2half_rn( q[ (size_t)col * d + h * 64 + ( lane & 7 ) * 8 + e ] ) );
+		const float lmax = kStreamScores( u, K4, nkv, qf, sp, warp, lane );
+		softmaxRow<ctaSync>( sp, nkv, lmax, sred, tid, warp, lane );
 		ptx::cp_async_wait_all();
 		__syncthreads();
-
-		const __half* sv = reinterpret_cast<const __half*>( ca_smem );
-		if( refThreads > 0 )
-		{
-			// reference arithmetic (see pvChainF16): one f16 chain per (reference thread, output dim), V read from shared memory
-			float* sof = &so[ 0 ][ 0 ][ 0 ];   // reused as [refThreads][64]
-			const int dc = ( T + refThreads - 1 ) / refThreads;
-			for( int idx = tid; idx < refThreads * 64; idx += CA_THREADS )
-			{
-				const int part = idx >> 6, e = idx & 63;
-				const int j0 = min( part * dc, T ), j1 = min( ( part + 1 ) * dc, T );
-				sof[ idx ] = pvChainF16( sp, sv + e, 64, j0, j1 );
-			}
-			__syncthreads();
-			if( tid < 64 )
-			{
-				float acc = sof[ tid ];
-				for( int k = 1; k < refThreads; k++ ) acc += sof[ k * 64 + tid ];
-				out[ (size_t)col * d + h * 64 + tid ] = __float2half_rn( acc );
-			}
-			return;
-		}
-
-		// exact mode: f32 accumulation
-		float o[ 8 ] = { 0, 0, 0, 0, 0, 0, 0, 0 };
-		const uint4* sv4 = reinterpret_cast<const uint4*>( ca_smem );
-		for( int j = warp * 4 + rgrp; j < T; j += ( CA_THREADS / 32 ) * 4 )
-		{
-			const float p = sp[ j ];
-			const uint4 u = sv4[ (size_t)j * 8 + sub ];
-			const __half2* h2 = reinterpret_cast<const __half2*>( &u );
-#pragma unroll
-			for( int e = 0; e < 4; e++ )
-			{
-				const float2 f = __half22float2( h2[ e ] );
-				o[ e * 2 ] += p * f.x;
-				o[ e * 2 + 1 ] += p * f.y;
-			}
-		}
-#pragma unroll
-		for( int e = 0; e < 8; e++ ) so[ warp ][ rgrp ][ sub * 8 + e ] = o[ e ];
-		__syncthreads();
-		if( tid < 64 )
-		{
-			float acc = 0.0f;
-			for( int w = 0; w < CA_THREADS / 32; w++ )
-#pragma unroll
-				for( int r = 0; r < 4; r++ ) acc += so[ w ][ r ][ tid ];
-			out[ (size_t)col * d + h * 64 + tid ] = __float2half_rn( acc );
-		}
+		pvSplitF16( sp, reinterpret_cast<const __half*>( at_smem ), nkv, refThreads, ( nkvAll + refThreads - 1 ) / refThreads, so,
+			out + (size_t)col * d + h * 64, tid );
 	}
-	static PerDeviceMax g_crossAttr;
-	static cudaError_t crossPrepare( int T )
+	static PerDeviceMax g_attnAttr;
+	static cudaError_t attnPrepare()
 	{
-		return g_crossAttr.raise( (size_t)T * 128, []( size_t n ) { return cudaFuncSetAttribute( cross_attn_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)n ); } );
+		return g_attnAttr.raise( 1, []( size_t ) {
+			cudaError_t e = cudaFuncSetAttribute( attn_decode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, attnMaxRows<false> * 128 );
+			if( e != cudaSuccess ) return e;
+			return cudaFuncSetAttribute( attn_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, attnMaxRows<true> * 128 );
+		} );
+	}
+	template<bool SELF>
+	static cudaError_t attnDecode( const float* q, const __half* kMem, const __half* vMem, __half* out, int B, int N, int H, int d, int rows, const int* dNPast, int refThreads, cudaStream_t s )
+	{
+		if( rows < 1 || rows > attnMaxRows<SELF> || refThreads < 1 || refThreads > kMaxRefThreads ) return cudaErrorInvalidValue;
+		return launchPdl( attn_decode_kernel<SELF>, dim3( B * H, N ), dim3( kAttnThreads ), (size_t)rows * 128, s, q, kMem, vMem, out, N, H, d, rows, dNPast, refThreads );
+	}
+	cudaError_t selfAttnDecode( const float* q, const __half* kCache, const __half* vCache, __half* out, int B, int N, int H, int d, int nTextCtx, const int* dNPast, int refThreads, cudaStream_t s )
+	{
+		return attnDecode<true>( q, kCache, vCache, out, B, N, H, d, nTextCtx, dNPast, refThreads, s );
 	}
 	cudaError_t crossAttnDecode( const float* q, const __half* kMem, const __half* vMem, __half* out, int B, int N, int H, int d, int T, int refThreads, cudaStream_t s )
 	{
-		if( T > CA_MAXT || refThreads < 0 || refThreads > PV_MAX_THREADS ) return cudaErrorInvalidValue;
-		cudaError_t e = crossPrepare( T );
-		if( e != cudaSuccess ) return e;
-		dim3 grid( B * H, N );
-		return launchPdl( cross_attn_decode_kernel, grid, dim3( CA_THREADS ), (size_t)T * 128, s, q, kMem, vMem, out, N, H, d, T, refThreads );
+		return attnDecode<false>( q, kMem, vMem, out, B, N, H, d, T, nullptr, refThreads, s );
 	}
 
 	// ---------------------------------------------------------------------------------------------------------------
