@@ -13,6 +13,7 @@
  *   wsp_set_mel               Whisper/source/whisper.h:107 whisper_set_mel
  *   wsp_encode                Whisper/source/whisper.h:117 whisper_encode          (Whisper/Whisper/WhisperContext.cpp:310 encode)
  *   wsp_set_audio_ctx         Whisper/API/sFullParams.h:75 sFullParams::audio_ctx  (whisper_context::exp_n_audio_ctx, Whisper/source/whisper.cpp:2836)
+ *   wsp_set_speed_up          Whisper/API/sFullParams.h:33 eFullParamsFlags::SpeedupAudio (whisper_pcm_to_mel_phase_vocoder, Whisper/source/whisper.cpp:2299-2311)
  *   wsp_decode                Whisper/source/whisper.h:128 whisper_decode + :140-150 whisper_sample_best/timestamp
  *                             (Whisper/Whisper/WhisperContext.cpp:578 decode, Whisper/Whisper/ContextImpl.cpp:71-157 sampleBest)
  *   wsp_get_logits/probs      Whisper/source/whisper.h:166 whisper_get_probs
@@ -111,7 +112,8 @@ wsp_status wsp_synchronize( wsp_context* c );
 /* device memory held by the context: workspaces, KV caches, mel slots (ContextImpl::getMemoryUse, Whisper/Whisper/ContextImpl.misc.cpp:170-182) */
 uint64_t wsp_context_device_bytes( const wsp_context* c );
 
-/* a1: 16 kHz mono f32 PCM (host) -> log-mel of chunk slot `slot`, kept on the device.  n_len = n_samples / 160 frames. */
+/* a1: 16 kHz mono f32 PCM (host) -> log-mel of chunk slot `slot`, kept on the device.  n_len = n_samples / 160 frames
+ * (n_samples / 320 with wsp_set_speed_up). */
 wsp_status wsp_pcm_to_mel( wsp_context* c, int32_t slot, const float* pcm, int32_t n_samples );
 /* a1, streamed flavour (iContext::runStreamed): log-mel of frames [0, n_frames) of `pcm` — which should extend 240 samples past the
  * last frame unless the stream ends there — normalised by the maximum over these frames only, floored at 1e-20; `forced_max` (may be
@@ -134,6 +136,17 @@ wsp_status wsp_encode( wsp_context* c, const int32_t* mel_offsets, int32_t batch
  * every decode attends over the n of the last encode, so the cross-KV layout and the decoder always agree.  wsp_get_tensor shapes
  * follow that encode: "enc.input" [2n][80], "enc.conv1" [2n][d], "enc.x" / "encode-out" [n][d], "cross_k" / "cross_v" [L][H][n][64]. */
 wsp_status wsp_set_audio_ctx( wsp_context* c, int32_t n );
+
+/* whisper_full_params::speed_up (Whisper/API/sFullParams.h:33 eFullParamsFlags::SpeedupAudio): on = 1 computes whole-clip log-mels with
+ * the reference's phase vocoder, whisper_pcm_to_mel_phase_vocoder (Whisper/source/whisper.cpp:2299-2311, 2060-2181 with speed_up): an
+ * 800-point Hann window and transform every 320 samples, the power spectrum's adjacent bins averaged back onto the model's 201 bins.
+ * The spectrum is compressed 2x in frequency, so the mel reads like audio played twice as fast: n_len = n_samples / 320 frames and one
+ * 3000-frame encoder window covers 60 s of audio (reduced accuracy, as the reference's -su option says).  on = 0 (the default) is the
+ * 400-point transform; any other value is WSP_E_INVALIDARG.  The value is context state and takes effect at the next log-mel of
+ * wsp_pcm_to_mel, wsp_run_chunks and wsp_run_chunks_resident; wsp_mel_len, wsp_get_mel and wsp_get_tensor("mel") follow that mel.
+ * While it is on, wsp_pcm_to_mel_window returns WSP_E_NOTIMPL (the reference has no streamed phase-vocoder window); wsp_set_mel is
+ * unaffected. */
+wsp_status wsp_set_speed_up( wsp_context* c, int32_t on );
 
 /* a13-a18: one decoder call for `batch` chunks, n_tokens new tokens each (tokens[b*n_tokens + i]), after n_past cached ones.
  * sampled (nullable) receives the greedy choice per chunk from the last token's distribution. */

@@ -36,7 +36,7 @@ EXPORTS = [
     "wsp_model_is_multilingual", "wsp_model_file_data", "wsp_model_meta_serialize", "wsp_model_from_meta",
     "wsp_engine_create", "wsp_engine_create_from_image", "wsp_engine_destroy", "wsp_engine_weight_bytes",
     "wsp_context_create", "wsp_context_destroy", "wsp_synchronize",
-    "wsp_context_device_bytes", "wsp_pcm_to_mel", "wsp_pcm_to_mel_window", "wsp_set_mel", "wsp_mel_len", "wsp_get_mel", "wsp_encode", "wsp_set_audio_ctx", "wsp_decode", "wsp_get_logits", "wsp_get_probs",
+    "wsp_context_device_bytes", "wsp_pcm_to_mel", "wsp_pcm_to_mel_window", "wsp_set_mel", "wsp_mel_len", "wsp_get_mel", "wsp_encode", "wsp_set_audio_ctx", "wsp_set_speed_up", "wsp_decode", "wsp_get_logits", "wsp_get_probs",
     "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_upload_pcm", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
     "wsp_host_alloc", "wsp_host_free", "wsp_timings",
     "wsp_replicas_create", "wsp_replicas_count", "wsp_replicas_run_chunks", "wsp_replicas_debug_fail_next", "wsp_replicas_destroy",
@@ -96,6 +96,7 @@ def lib():
     sig("wsp_get_mel", i32, [vp, i32, fp, sz])
     sig("wsp_encode", i32, [vp, ip, i32])
     sig("wsp_set_audio_ctx", i32, [vp, i32])
+    sig("wsp_set_speed_up", i32, [vp, i32])
     sig("wsp_decode", i32, [vp, ip, i32, i32, i32, u32, C.POINTER(TokenData)])
     sig("wsp_get_logits", i32, [vp, fp, sz])
     sig("wsp_get_probs", i32, [vp, fp, sz])
@@ -276,6 +277,11 @@ class Context:
         """sFullParams::audio_ctx: the next encode covers only the first n audio positions (2n mel frames); n <= 0 = the model's
         n_audio_ctx.  Decodes attend over the n of the last encode."""
         check(self.L.wsp_set_audio_ctx(self.h, int(n)))
+
+    def set_speed_up(self, on):
+        """whisper_full_params::speed_up: whole-clip log-mels (pcm_to_mel, run_chunks*) through the reference's 2x phase vocoder,
+        n_samples // 320 frames, so a 3000-frame window holds 60 s of audio.  Takes 0 or 1 (bools are accepted)."""
+        check(self.L.wsp_set_speed_up(self.h, int(on)))
 
     def decode(self, tokens, n_past: int, batch: int = 1, flags: int = 0):
         """tokens: [batch][n_tokens] (or None with DECODE_DEVICE_TOKENS).  Returns list of sampled dicts (or None)."""

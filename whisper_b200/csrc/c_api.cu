@@ -370,6 +370,11 @@ wsp_status wsp_set_audio_ctx( wsp_context* c, int32_t n )
 	if( !c ) return fail( WSP_E_POINTER, "context" );
 	return ctxSetAudioCtx( *c->c, n );
 }
+wsp_status wsp_set_speed_up( wsp_context* c, int32_t on )
+{
+	if( !c ) return fail( WSP_E_POINTER, "context" );
+	return ctxSetSpeedUp( *c->c, on );
+}
 wsp_status wsp_debug_set_encoder_layers( wsp_context* c, int32_t n )
 {
 	if( !c ) return fail( WSP_E_POINTER, "context" );

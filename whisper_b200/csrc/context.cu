@@ -190,12 +190,17 @@ namespace wsp
 		return WSP_OK;
 	}
 
+	// frames of the whole-clip log-mel of nSamples samples: n / hop (whisper.cpp:2080), hop 160 for whisper_pcm_to_mel and 320 for the
+	// phase vocoder of whisper_pcm_to_mel_phase_vocoder (:2299-2311) that speed-up selects
+	static int melFrames( const Context& c, int nSamples ) { return nSamples / ( c.speedUp ? 320 : 160 ); }
+	static const kern::MelTables& melTables( const Context& c ) { return c.speedUp ? c.e->melVocoder : c.e->mel; }
+
 	static int melFromDevicePcm( Context& c, int slot, const float* pcmDev, int nSamples )
 	{
-		const int nLen = nSamples / 160;   // whisper.cpp:2080
+		const int nLen = melFrames( c, nSamples );
 		WSP_CHECK( ensureMelSlot( c, slot, nLen ) );
 		MelSlot& s = c.slots[ slot ];
-		WSP_CUDA( kern::melPower( c.e->mel, pcmDev, nSamples, nLen, s.mel, c.melMax + slot, c.stream ) );
+		WSP_CUDA( kern::melPower( melTables( c ), pcmDev, nSamples, nLen, s.mel, c.melMax + slot, c.speedUp, c.stream ) );
 		WSP_CUDA( kern::melNormalize( s.mel, 80 * nLen, c.melMax + slot, c.stream ) );
 		launched( 3 );
 		return WSP_OK;
@@ -213,13 +218,14 @@ namespace wsp
 			for( int i = 0; i < mb.count; i++ )
 			{
 				const int n = samplesOf( b0 + i );
-				WSP_CHECK( ensureMelSlot( c, b0 + i, n / 160 ) );   // whisper.cpp:2080
+				const int nLen = melFrames( c, n );
+				WSP_CHECK( ensureMelSlot( c, b0 + i, nLen ) );
 				mb.pcm[ i ] = pcmOf( b0 + i );
 				mb.mel[ i ] = c.slots[ b0 + i ].mel;
 				mb.nSamples[ i ] = n;
-				mb.nLen[ i ] = n / 160;
+				mb.nLen[ i ] = nLen;
 			}
-			WSP_CUDA( kern::melBatch( c.e->mel, mb, c.stream ) );
+			WSP_CUDA( kern::melBatch( melTables( c ), mb, c.speedUp, c.stream ) );
 			launched( 3 );
 		}
 		return WSP_OK;
@@ -260,6 +266,8 @@ namespace wsp
 	int ctxPcmToMelWindow( Context& c, int slot, const float* pcmHost, int nSamples, int nFrames, const float* forcedMax, float* maxOut )
 	{
 		if( ( !pcmHost && nSamples != 0 ) || nSamples < 0 || nFrames < 0 ) return fail( WSP_E_INVALIDARG, "pcm / frame count" );
+		// the reference streams only the 400-point transform (MelStreamer.cpp); it has no streamed phase-vocoder window to follow
+		if( c.speedUp ) return fail( WSP_E_NOTIMPL, "no streamed log-mel window with speed-up on" );
 		WSP_CUDA( cudaSetDevice( c.e->device ) );
 		WSP_CHECK( ensurePcm( c, (size_t)( nSamples > 0 ? nSamples : 1 ) ) );
 		WSP_CHECK( ensureMelSlot( c, slot, nFrames ) );
@@ -267,7 +275,7 @@ namespace wsp
 		WSP_CUDA( cudaEventRecord( c.ev[ 0 ], c.stream ) );
 		if( nSamples > 0 )
 			WSP_CUDA( cudaMemcpyAsync( c.pcmDev, pcmHost, (size_t)nSamples * 4, cudaMemcpyHostToDevice, c.stream ) );
-		WSP_CUDA( kern::melPower( c.e->mel, c.pcmDev, nSamples, nFrames, s.mel, c.melMax + slot, c.stream ) );
+		WSP_CUDA( kern::melPower( c.e->mel, c.pcmDev, nSamples, nFrames, s.mel, c.melMax + slot, false, c.stream ) );
 		int32_t ordered = 0;
 		WSP_CUDA( cudaMemcpyAsync( &ordered, c.melMax + slot, 4, cudaMemcpyDeviceToHost, c.stream ) );
 		WSP_CUDA( cudaStreamSynchronize( c.stream ) );
@@ -399,6 +407,14 @@ namespace wsp
 	{
 		if( n > c.e->hp.n_audio_ctx ) return fail( WSP_E_INVALIDARG, "audio_ctx exceeds the model's n_audio_ctx" );
 		c.audioCtx = n > 0 ? n : 0;
+		return WSP_OK;
+	}
+
+	// whisper_full_params::speed_up (sFullParams.h:33 SpeedupAudio): whole-clip log-mels through the phase vocoder
+	int ctxSetSpeedUp( Context& c, int on )
+	{
+		if( on != 0 && on != 1 ) return fail( WSP_E_INVALIDARG, "speed-up must be 0 or 1" );
+		c.speedUp = on != 0;
 		return WSP_OK;
 	}
 

@@ -289,6 +289,24 @@ namespace wsp
 			WSP_CUDA( cudaMemcpy( df, m.filters.data(), m.filters.size() * 4, cudaMemcpyHostToDevice ) );
 			e->mel.hann = dh; e->mel.cosT = dc; e->mel.sinT = ds; e->mel.filters = df;
 		}
+		// ---- the phase vocoder's 800-point window and twiddles (speed-up: log_mel_spectrogram with fft_size 800, whisper.cpp:2076, 2303) ----
+		{
+			std::vector<float> hann( 800 );
+			std::vector<double2> tw( 800 );
+			for( int i = 0; i < 800; i++ )
+			{
+				hann[ i ] = (float)( 0.5 * ( 1.0 - cos( ( 2.0 * M_PI * i ) / 800.0 ) ) );
+				tw[ i ] = make_double2( cos( 2.0 * M_PI * i / 800.0 ), sin( 2.0 * M_PI * i / 800.0 ) );
+			}
+			float* dh = up.alloc<float>( 800 );
+			double2* dt = up.alloc<double2>( 800 );
+			if( !dh || !dt ) return fail( WSP_E_OUTOFMEMORY, "weight arena" );
+			WSP_CUDA( cudaMemcpy( dh, hann.data(), 800 * 4, cudaMemcpyHostToDevice ) );
+			WSP_CUDA( cudaMemcpy( dt, tw.data(), 800 * sizeof( double2 ), cudaMemcpyHostToDevice ) );
+			e->melVocoder = e->mel;
+			e->melVocoder.hann = dh; e->melVocoder.twiddle = dt;
+			e->melVocoder.cosT = e->melVocoder.sinT = nullptr;
+		}
 		WSP_CUDA( cudaDeviceSynchronize() );
 		*out = e.release();
 		return WSP_OK;

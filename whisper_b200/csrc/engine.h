@@ -80,6 +80,7 @@ namespace wsp
 		LnW decLn;
 		std::vector<DecLayerW> dec;
 		kern::MelTables mel;
+		kern::MelTables melVocoder;   // the phase vocoder's 800-point window and twiddles, mel's filters (speed-up)
 
 		~Engine();
 	};
@@ -115,6 +116,7 @@ namespace wsp
 		int* melMax = nullptr;          // [maxB] ordered-int maxima
 		float* pcmDev = nullptr; size_t pcmCap = 0;
 		uint64_t devBytes = 0;          // device memory this context holds (timingsPrint's memory table)
+		bool speedUp = false;           // whole-clip log-mels through the 2x phase vocoder (wsp_set_speed_up)
 
 		// encoder workspaces
 		// sized for n_audio_ctx = 1500; an encode over n <= 1500 audio positions (audio_ctx) packs its chunks densely with n in
@@ -202,6 +204,7 @@ namespace wsp
 	int ctxSetMel( Context& c, int slot, const float* melHost, int nLen );
 	int ctxEncode( Context& c, const int32_t* offsets, int batch );
 	int ctxSetAudioCtx( Context& c, int n );
+	int ctxSetSpeedUp( Context& c, int on );
 	int ctxDecode( Context& c, const int32_t* tokensHost, int nTokens, int nPast, int batch, uint32_t flags, wsp_token_data* sampledHost );
 	int ctxUploadPcm( Context& c, int slot, const float* pcmHost, int nSamples );
 	int ctxProfileDecode( Context& c, int batch, int nSteps, float* msByKind, int* launchesByKind );

@@ -35,6 +35,8 @@ namespace kern
 		const double2* twiddle = nullptr; // [400]  { cosT, sinT } interleaved: one 16-byte shared-memory read per DFT term
 		const short2* band = nullptr;     // [80]   [x, y) = the bins where the band's filter row is non-zero (real filter banks are triangular)
 	};
+	// The phase vocoder (speed-up, whisper.cpp:2299-2311) takes a second MelTables of the same layout: hann [800] and twiddle [800] of the
+	// 800-point transform, cosT / sinT unset, filters and band shared with the 400-point tables.
 	// pcm [nSamples] -> raw log10 mel [80][nLen] (row = band) and the running maximum (ordered-int encoded float) in *maxSlot
 	// up to MEL_BATCH chunks transformed and normalised by one launch each (power, normalise); maxSlots[b] is chunk b's maximum
 	constexpr int MEL_BATCH = 16;
@@ -47,8 +49,9 @@ namespace kern
 		int* maxSlots;                 // [count] consecutive
 		int count;
 	};
-	cudaError_t melBatch( const MelTables& tb, const MelBatch& mb, cudaStream_t s );
-	cudaError_t melPower( const MelTables& tb, const float* pcm, int nSamples, int nLen, float* melRaw, int* maxSlot, cudaStream_t s );
+	// speedUp: the phase vocoder (800-point transform, hop 320, tb = its tables) instead of the 400-point one (hop 160)
+	cudaError_t melBatch( const MelTables& tb, const MelBatch& mb, bool speedUp, cudaStream_t s );
+	cudaError_t melPower( const MelTables& tb, const float* pcm, int nSamples, int nLen, float* melRaw, int* maxSlot, bool speedUp, cudaStream_t s );
 	// in place: clamp to (max - 8), (x + 4) / 4
 	cudaError_t melNormalize( float* mel, int count, const int* maxSlot, cudaStream_t s );
 	// mel f32 [80][nLen] at frame offset -> time-major f16 window [1 + frames + 1][80], halo rows (conv padding) written as zeros;

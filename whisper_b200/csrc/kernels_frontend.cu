@@ -19,59 +19,66 @@ namespace kern
 	//   mel[j] = sum_k folded[k]*filters[j][k] in double ; log10(max(., 1e-10)) -> float.
 	// The oracle's recursive f32 FFT (:2009-2056) is replaced by a direct 201-bin DFT with f64 accumulation: exact to f32
 	// rounding, so the only difference to the oracle is the oracle's own f32 FFT round-off.
-	constexpr int MEL_FFT = 400;
-	constexpr int MEL_HOP = 160;
+	// FFT = 800 is the phase vocoder of whisper_pcm_to_mel_phase_vocoder (:2299-2311, speed_up = true): hop 320, an 800-point
+	// Hann window and DFT, the same fold over bins 1..399 (bin 400 single, bin 401 = |X399|^2 left unfolded because the loop stops
+	// at 399), then adjacent bins averaged onto the model's 201: P'[j] = 0.5 * (P[2j] + P[2j+1]) (:2130-2135).
 	constexpr int MEL_BINS = 201;
 	constexpr int MEL_BANDS = 80;
+	template<int FFT> struct MelGeom;
+	template<> struct MelGeom<400> { static constexpr int HOP = 160, THREADS = 256; };
+	template<> struct MelGeom<800> { static constexpr int HOP = 320, THREADS = 512; };
 
+	template<int FFT>
 	__device__ __forceinline__ void melFrame( const MelTables& tb, const float* __restrict__ pcm, int nSamples, int nLen, float* __restrict__ melRaw, int* maxSlot, const int frame )
 	{
-		__shared__ float sx[ MEL_FFT ];
-		__shared__ double2 stw[ MEL_FFT ];          // { cos, sin }( 2 pi m / 400 )
-		__shared__ double sA[ 2 ][ MEL_FFT / 4 ];   // [k parity][n]: cosine-side combinations
-		__shared__ double sB[ 2 ][ MEL_FFT / 4 ];   //                 sine-side combinations
-		__shared__ float sp[ MEL_BINS + 7 ];
-		__shared__ float smax[ 8 ];
+		constexpr int NBINS = FFT / 2 + 1;         // DFT bins computed: 201 | 401
+		constexpr int NWARPS = MelGeom<FFT>::THREADS / 32;
+		__shared__ float sx[ FFT ];
+		__shared__ double2 stw[ FFT ];          // { cos, sin }( 2 pi m / FFT )
+		__shared__ double sA[ 2 ][ FFT / 4 ];   // [k parity][n]: cosine-side combinations
+		__shared__ double sB[ 2 ][ FFT / 4 ];   //                 sine-side combinations
+		__shared__ float sp[ NBINS + 7 ];
+		__shared__ float smax[ NWARPS ];
 		const int tid = threadIdx.x;
-		const int offset = frame * MEL_HOP;
-		for( int n = tid; n < MEL_FFT; n += blockDim.x )
+		const int offset = frame * MelGeom<FFT>::HOP;
+		for( int n = tid; n < FFT; n += blockDim.x )
 		{
 			const int idx = offset + n;
 			sx[ n ] = idx < nSamples ? tb.hann[ n ] * pcm[ idx ] : 0.0f;
 			stw[ n ] = tb.twiddle[ n ];
 		}
 		__syncthreads();
-		// Real 400-point DFT in a quarter of the multiply-adds.  With w = exp(-2 pi i k / 400):
-		//   X[k] = sum_{n<200} y[n] w^n,  y[n] = x[n] + (-1)^k x[n+200]           (w^200 = (-1)^k)
-		//        = y[0] + y[100] (-i)^k + sum_{n=1..99} ( y[n] w^n + (-1)^k y[200-n] conj(w^n) )
-		//   Re = y[0] + Re(y[100] (-i)^k) + sum cos(t_n) A[n],   A[n] = y[n] + (-1)^k y[200-n]
-		//   Im =        Im(y[100] (-i)^k) - sum sin(t_n) B[n],   B[n] = y[n] - (-1)^k y[200-n]
-		// (f64 accumulation as before; only the summation order differs from the plain 400-term sum)
-		constexpr int Q = MEL_FFT / 4;   // 100
+		// Real FFT-point DFT in a quarter of the multiply-adds (Q = FFT / 4).  With w = exp(-2 pi i k / FFT):
+		//   X[k] = sum_{n<2Q} y[n] w^n,  y[n] = x[n] + (-1)^k x[n+2Q]           (w^2Q = (-1)^k)
+		//        = y[0] + y[Q] (-i)^k + sum_{n=1..Q-1} ( y[n] w^n + (-1)^k y[2Q-n] conj(w^n) )
+		//   Re = y[0] + Re(y[Q] (-i)^k) + sum cos(t_n) A[n],   A[n] = y[n] + (-1)^k y[2Q-n]
+		//   Im =        Im(y[Q] (-i)^k) - sum sin(t_n) B[n],   B[n] = y[n] - (-1)^k y[2Q-n]
+		// (f64 accumulation as before; only the summation order differs from the plain FFT-term sum)
+		constexpr int Q = FFT / 4;   // 100 | 200
 		if( tid < 2 * Q )
 		{
 			const int par = tid / Q, n = tid - par * Q;
 			const double sg = par ? -1.0 : 1.0;
 			const double yn = (double)sx[ n ] + sg * (double)sx[ n + 2 * Q ];
-			const double ym = n == 0 ? 0.0 : (double)sx[ 2 * Q - n ] + sg * (double)sx[ 4 * Q - n ];   // y[200-n]
+			const double ym = n == 0 ? 0.0 : (double)sx[ 2 * Q - n ] + sg * (double)sx[ 4 * Q - n ];   // y[2Q-n]
 			sA[ par ][ n ] = yn + sg * ym;
 			sB[ par ][ n ] = yn - sg * ym;
 		}
 		__syncthreads();
-		if( tid < MEL_BINS )
+		if( tid < NBINS )
 		{
 			const int k = tid;
 			const int par = k & 1;
 			const double sg = par ? -1.0 : 1.0;
 			const double y0 = (double)sx[ 0 ] + sg * (double)sx[ 2 * Q ];
-			const double y100 = (double)sx[ Q ] + sg * (double)sx[ 3 * Q ];
+			const double yQ = (double)sx[ Q ] + sg * (double)sx[ 3 * Q ];
 			double re = y0, im = 0.0;
-			switch( k & 3 )   // y[100] * (-i)^k
+			switch( k & 3 )   // y[Q] * (-i)^k
 			{
-			case 0: re += y100; break;
-			case 1: im -= y100; break;
-			case 2: re -= y100; break;
-			default: im += y100; break;
+			case 0: re += yQ; break;
+			case 1: im -= yQ; break;
+			case 2: re -= yQ; break;
+			default: im += yQ; break;
 			}
 			const double* A = sA[ par ];
 			const double* Bv = sB[ par ];
@@ -83,11 +90,13 @@ namespace kern
 				re += A[ n ] * w.x;
 				im -= Bv[ n ] * w.y;
 				idx += k;
-				if( idx >= MEL_FFT ) idx -= MEL_FFT;
+				if( idx >= FFT ) idx -= FFT;
 			}
 			const float fr = (float)re, fi = (float)im;
 			float pw = fr * fr + fi * fi;
-			if( k > 0 && k < MEL_FFT / 2 ) pw = pw + pw;   // fft_out[j] += fft_out[400 - j]  (whisper.cpp:2118-2123)
+			if constexpr( FFT == 800 )
+				if( k == FFT / 2 - 1 ) sp[ FFT / 2 + 1 ] = pw;   // bin 401 = |X401|^2 = |X399|^2, not folded
+			if( k > 0 && k < FFT / 2 ) pw = pw + pw;   // fft_out[j] += fft_out[FFT - j]  (whisper.cpp:2118-2123)
 			sp[ k ] = pw;
 		}
 		__syncthreads();
@@ -98,7 +107,12 @@ namespace kern
 			const short2 range = tb.band[ tid ];   // outside it the filter row is exactly zero: those terms add +0.0
 			double sum = 0.0;
 			for( int k = range.x; k < range.y; k++ )
-				sum += (double)( sp[ k ] * f[ k ] );   // float product, double accumulate (whisper.cpp:2139-2143)
+			{
+				float p = sp[ k ];
+				if constexpr( FFT == 800 )
+					p = (float)( 0.5 * (double)( sp[ 2 * k ] + sp[ 2 * k + 1 ] ) );   // whisper.cpp:2133, f32 sum, double half
+				sum += (double)( p * f[ k ] );   // float product, double accumulate (whisper.cpp:2139-2143)
+			}
 			if( sum < 1e-10 ) sum = 1e-10;
 			v = (float)log10( sum );
 			melRaw[ (size_t)tid * nLen + frame ] = v;
@@ -115,18 +129,20 @@ namespace kern
 		}
 	}
 
-	__global__ void __launch_bounds__( 256 )
+	template<int FFT>
+	__global__ void __launch_bounds__( MelGeom<FFT>::THREADS )
 		mel_power_kernel( MelTables tb, const float* __restrict__ pcm, int nSamples, int nLen, float* __restrict__ melRaw, int* maxSlot )
 	{
-		melFrame( tb, pcm, nSamples, nLen, melRaw, maxSlot, blockIdx.x );
+		melFrame<FFT>( tb, pcm, nSamples, nLen, melRaw, maxSlot, blockIdx.x );
 	}
 	// the same for up to MEL_BATCH chunks in one launch: blockIdx.y = chunk (the driver loop of BASELINE.md §2 transforms B chunks per step)
-	__global__ void __launch_bounds__( 256 )
+	template<int FFT>
+	__global__ void __launch_bounds__( MelGeom<FFT>::THREADS )
 		mel_power_batch_kernel( MelTables tb, MelBatch mb )
 	{
 		const int b = blockIdx.y;
 		if( (int)blockIdx.x >= mb.nLen[ b ] ) return;
-		melFrame( tb, mb.pcm[ b ], mb.nSamples[ b ], mb.nLen[ b ], mb.mel[ b ], mb.maxSlots + b, blockIdx.x );
+		melFrame<FFT>( tb, mb.pcm[ b ], mb.nSamples[ b ], mb.nLen[ b ], mb.mel[ b ], mb.maxSlots + b, blockIdx.x );
 	}
 
 	__device__ __forceinline__ void melNormOne( float* mel, int i, const int* maxSlot )
@@ -153,14 +169,19 @@ namespace kern
 
 	__global__ void init_max_kernel( int* maxSlot ) { maxSlot[ threadIdx.x ] = orderedFromFloat( -1e20f ); }
 
-	cudaError_t melPower( const MelTables& tb, const float* pcm, int nSamples, int nLen, float* melRaw, int* maxSlot, cudaStream_t s )
+	cudaError_t melPower( const MelTables& tb, const float* pcm, int nSamples, int nLen, float* melRaw, int* maxSlot, bool speedUp, cudaStream_t s )
 	{
 		init_max_kernel<<<1, 1, 0, s>>>( maxSlot );
 		if( nLen > 0 )
-			mel_power_kernel<<<nLen, 256, 0, s>>>( tb, pcm, nSamples, nLen, melRaw, maxSlot );
+		{
+			if( speedUp )
+				mel_power_kernel<800><<<nLen, MelGeom<800>::THREADS, 0, s>>>( tb, pcm, nSamples, nLen, melRaw, maxSlot );
+			else
+				mel_power_kernel<400><<<nLen, MelGeom<400>::THREADS, 0, s>>>( tb, pcm, nSamples, nLen, melRaw, maxSlot );
+		}
 		return cudaGetLastError();
 	}
-	cudaError_t melBatch( const MelTables& tb, const MelBatch& mb, cudaStream_t s )
+	cudaError_t melBatch( const MelTables& tb, const MelBatch& mb, bool speedUp, cudaStream_t s )
 	{
 		if( mb.count < 1 || mb.count > MEL_BATCH ) return cudaErrorInvalidValue;
 		int maxLen = 0;
@@ -168,7 +189,10 @@ namespace kern
 		init_max_kernel<<<1, mb.count, 0, s>>>( mb.maxSlots );
 		if( maxLen > 0 )
 		{
-			mel_power_batch_kernel<<<dim3( maxLen, mb.count ), 256, 0, s>>>( tb, mb );
+			if( speedUp )
+				mel_power_batch_kernel<800><<<dim3( maxLen, mb.count ), MelGeom<800>::THREADS, 0, s>>>( tb, mb );
+			else
+				mel_power_batch_kernel<400><<<dim3( maxLen, mb.count ), MelGeom<400>::THREADS, 0, s>>>( tb, mb );
 			mel_norm_batch_kernel<<<dim3( ( MEL_BANDS * maxLen + 255 ) / 256, mb.count ), 256, 0, s>>>( mb );
 		}
 		return cudaGetLastError();
