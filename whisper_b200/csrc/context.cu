@@ -195,37 +195,28 @@ namespace wsp
 	static int melFrames( const Context& c, int nSamples ) { return nSamples / ( c.speedUp ? 320 : 160 ); }
 	static const kern::MelTables& melTables( const Context& c ) { return c.speedUp ? c.e->melVocoder : c.e->mel; }
 
-	static int melFromDevicePcm( Context& c, int slot, const float* pcmDev, int nSamples )
-	{
-		const int nLen = melFrames( c, nSamples );
-		WSP_CHECK( ensureMelSlot( c, slot, nLen ) );
-		MelSlot& s = c.slots[ slot ];
-		WSP_CUDA( kern::melPower( melTables( c ), pcmDev, nSamples, nLen, s.mel, c.melMax + slot, c.speedUp, c.stream ) );
-		WSP_CUDA( kern::melNormalize( s.mel, 80 * nLen, c.melMax + slot, c.stream ) );
-		launched( 3 );
-		return WSP_OK;
-	}
-
-	// log-mel of chunks [0, batch) in one pair of launches per 16 chunks: pcmOf( b ) / samplesOf( b ) name chunk b's device PCM
+	// log-mel of chunks [0, batch) into slots [slot0, slot0 + batch), in one triple of launches per 16 chunks: pcmOf( b ) /
+	// samplesOf( b ) name chunk b's device PCM
 	template<class P, class N>
-	static int melBatchFromDevicePcm( Context& c, int batch, P pcmOf, N samplesOf )
+	static int melBatchFromDevicePcm( Context& c, int slot0, int batch, P pcmOf, N samplesOf )
 	{
 		for( int b0 = 0; b0 < batch; b0 += kern::MEL_BATCH )
 		{
 			kern::MelBatch mb{};
 			mb.count = batch - b0 < kern::MEL_BATCH ? batch - b0 : kern::MEL_BATCH;
-			mb.maxSlots = c.melMax + b0;
+			mb.maxSlots = c.melMax + slot0 + b0;
 			for( int i = 0; i < mb.count; i++ )
 			{
 				const int n = samplesOf( b0 + i );
 				const int nLen = melFrames( c, n );
-				WSP_CHECK( ensureMelSlot( c, b0 + i, nLen ) );
+				WSP_CHECK( ensureMelSlot( c, slot0 + b0 + i, nLen ) );
 				mb.pcm[ i ] = pcmOf( b0 + i );
-				mb.mel[ i ] = c.slots[ b0 + i ].mel;
+				mb.mel[ i ] = c.slots[ slot0 + b0 + i ].mel;
 				mb.nSamples[ i ] = n;
 				mb.nLen[ i ] = nLen;
 			}
-			WSP_CUDA( kern::melBatch( melTables( c ), mb, c.speedUp, c.stream ) );
+			WSP_CUDA( kern::melBatchPower( melTables( c ), mb, c.speedUp, c.stream ) );
+			WSP_CUDA( kern::melBatchNormalize( mb, c.stream ) );
 			launched( 3 );
 		}
 		return WSP_OK;
@@ -242,21 +233,30 @@ namespace wsp
 		return WSP_OK;
 	}
 
-	int ctxPcmToMel( Context& c, int slot, const float* pcmHost, int nSamples )
+	// one clip's host PCM into c.pcmDev, then melOf() enqueues its log-mel; both are timed as the mel stage
+	template<class M>
+	static int pcmToMelTimed( Context& c, const float* pcmHost, int nSamples, M melOf )
 	{
-		if( ( !pcmHost && nSamples != 0 ) || nSamples < 0 ) return fail( WSP_E_INVALIDARG, "pcm" );
 		WSP_CUDA( cudaSetDevice( c.e->device ) );
 		WSP_CHECK( ensurePcm( c, (size_t)( nSamples > 0 ? nSamples : 1 ) ) );
 		WSP_CUDA( cudaEventRecord( c.ev[ 0 ], c.stream ) );
 		if( nSamples > 0 )
 			WSP_CUDA( cudaMemcpyAsync( c.pcmDev, pcmHost, (size_t)nSamples * 4, cudaMemcpyHostToDevice, c.stream ) );
-		WSP_CHECK( melFromDevicePcm( c, slot, c.pcmDev, nSamples ) );
+		WSP_CHECK( melOf() );
 		WSP_CUDA( cudaEventRecord( c.ev[ 1 ], c.stream ) );
 		WSP_CUDA( cudaStreamSynchronize( c.stream ) );
 		float ms = 0;
 		cudaEventElapsedTime( &ms, c.ev[ 0 ], c.ev[ 1 ] );
 		c.ms[ 0 ] += ms; c.calls[ 0 ]++;
 		return WSP_OK;
+	}
+
+	int ctxPcmToMel( Context& c, int slot, const float* pcmHost, int nSamples )
+	{
+		if( ( !pcmHost && nSamples != 0 ) || nSamples < 0 ) return fail( WSP_E_INVALIDARG, "pcm" );
+		return pcmToMelTimed( c, pcmHost, nSamples, [ & ]() -> int {
+			return melBatchFromDevicePcm( c, slot, 1, [ & ]( int ) { return (const float*)c.pcmDev; }, [ & ]( int ) { return nSamples; } );
+		} );
 	}
 
 	// One window of a streamed clip (Whisper/Whisper/MelStreamer.cpp:128-236): frames [0, nFrames) of the PCM handed in — the PCM may
@@ -268,35 +268,33 @@ namespace wsp
 		if( ( !pcmHost && nSamples != 0 ) || nSamples < 0 || nFrames < 0 ) return fail( WSP_E_INVALIDARG, "pcm / frame count" );
 		// the reference streams only the 400-point transform (MelStreamer.cpp); it has no streamed phase-vocoder window to follow
 		if( c.speedUp ) return fail( WSP_E_NOTIMPL, "no streamed log-mel window with speed-up on" );
-		WSP_CUDA( cudaSetDevice( c.e->device ) );
-		WSP_CHECK( ensurePcm( c, (size_t)( nSamples > 0 ? nSamples : 1 ) ) );
-		WSP_CHECK( ensureMelSlot( c, slot, nFrames ) );
-		MelSlot& s = c.slots[ slot ];
-		WSP_CUDA( cudaEventRecord( c.ev[ 0 ], c.stream ) );
-		if( nSamples > 0 )
-			WSP_CUDA( cudaMemcpyAsync( c.pcmDev, pcmHost, (size_t)nSamples * 4, cudaMemcpyHostToDevice, c.stream ) );
-		WSP_CUDA( kern::melPower( c.e->mel, c.pcmDev, nSamples, nFrames, s.mel, c.melMax + slot, false, c.stream ) );
-		int32_t ordered = 0;
-		WSP_CUDA( cudaMemcpyAsync( &ordered, c.melMax + slot, 4, cudaMemcpyDeviceToHost, c.stream ) );
-		WSP_CUDA( cudaStreamSynchronize( c.stream ) );
-		// the device keeps the maximum as an order-preserving integer (kernels_frontend.cu: orderedFromFloat)
-		auto toFloat = []( int32_t i ) { const int32_t b = i >= 0 ? i : i ^ 0x7FFFFFFF; float f; memcpy( &f, &b, 4 ); return f; };
-		auto toOrdered = []( float f ) { int32_t b; memcpy( &b, &f, 4 ); return b >= 0 ? b : b ^ 0x7FFFFFFF; };
-		float mmax = toFloat( ordered );
-		if( !( mmax > 1e-20f ) ) mmax = 1e-20f;
-		if( maxOut ) *maxOut = mmax;
-		if( forcedMax ) mmax = *forcedMax;
-		const int32_t wanted = toOrdered( mmax );
-		if( wanted != ordered )
-			WSP_CUDA( cudaMemcpyAsync( c.melMax + slot, &wanted, 4, cudaMemcpyHostToDevice, c.stream ) );
-		WSP_CUDA( kern::melNormalize( s.mel, 80 * nFrames, c.melMax + slot, c.stream ) );
-		launched( 3 );
-		WSP_CUDA( cudaEventRecord( c.ev[ 1 ], c.stream ) );
-		WSP_CUDA( cudaStreamSynchronize( c.stream ) );
-		float ms = 0;
-		cudaEventElapsedTime( &ms, c.ev[ 0 ], c.ev[ 1 ] );
-		c.ms[ 0 ] += ms; c.calls[ 0 ]++;
-		return WSP_OK;
+		return pcmToMelTimed( c, pcmHost, nSamples, [ & ]() -> int {
+			WSP_CHECK( ensureMelSlot( c, slot, nFrames ) );
+			kern::MelBatch mb{};
+			mb.pcm[ 0 ] = c.pcmDev;
+			mb.mel[ 0 ] = c.slots[ slot ].mel;
+			mb.nSamples[ 0 ] = nSamples;
+			mb.nLen[ 0 ] = nFrames;
+			mb.maxSlots = c.melMax + slot;
+			mb.count = 1;
+			WSP_CUDA( kern::melBatchPower( c.e->mel, mb, false, c.stream ) );
+			int32_t ordered = 0;
+			WSP_CUDA( cudaMemcpyAsync( &ordered, c.melMax + slot, 4, cudaMemcpyDeviceToHost, c.stream ) );
+			WSP_CUDA( cudaStreamSynchronize( c.stream ) );
+			// the device keeps the maximum as an order-preserving integer (kernels_frontend.cu: orderedFromFloat)
+			auto toFloat = []( int32_t i ) { const int32_t b = i >= 0 ? i : i ^ 0x7FFFFFFF; float f; memcpy( &f, &b, 4 ); return f; };
+			auto toOrdered = []( float f ) { int32_t b; memcpy( &b, &f, 4 ); return b >= 0 ? b : b ^ 0x7FFFFFFF; };
+			float mmax = toFloat( ordered );
+			if( !( mmax > 1e-20f ) ) mmax = 1e-20f;
+			if( maxOut ) *maxOut = mmax;
+			if( forcedMax ) mmax = *forcedMax;
+			const int32_t wanted = toOrdered( mmax );
+			if( wanted != ordered )
+				WSP_CUDA( cudaMemcpyAsync( c.melMax + slot, &wanted, 4, cudaMemcpyHostToDevice, c.stream ) );
+			WSP_CUDA( kern::melBatchNormalize( mb, c.stream ) );
+			launched( 3 );
+			return WSP_OK;
+		} );
 	}
 
 	int ctxSetMel( Context& c, int slot, const float* melHost, int nLen )
@@ -713,7 +711,7 @@ namespace wsp
 			// inputs already in HBM (wsp_upload_pcm): the log-mel front end still runs inside the timed region
 			for( int b = 0; b < batch; b++ )
 				if( !c.slots[ b ].pcm ) return fail( WSP_E_INVALIDARG, "no resident PCM in slot " + std::to_string( b ) + " (call wsp_upload_pcm)" );
-			WSP_CHECK( melBatchFromDevicePcm( c, batch, [ & ]( int b ) { return (const float*)c.slots[ b ].pcm; }, [ & ]( int b ) { return c.slots[ b ].pcmSamples; } ) );
+			WSP_CHECK( melBatchFromDevicePcm( c, 0, batch, [ & ]( int b ) { return (const float*)c.slots[ b ].pcm; }, [ & ]( int b ) { return c.slots[ b ].pcmSamples; } ) );
 		}
 		else
 		{
@@ -729,7 +727,7 @@ namespace wsp
 				offs[ (size_t)b ] = off;
 				off += (size_t)nSamples[ b ];
 			}
-			WSP_CHECK( melBatchFromDevicePcm( c, batch, [ & ]( int b ) { return (const float*)( c.pcmDev + offs[ (size_t)b ] ); }, [ & ]( int b ) { return (int)nSamples[ b ]; } ) );
+			WSP_CHECK( melBatchFromDevicePcm( c, 0, batch, [ & ]( int b ) { return (const float*)( c.pcmDev + offs[ (size_t)b ] ); }, [ & ]( int b ) { return (int)nSamples[ b ]; } ) );
 		}
 		WSP_CUDA( cudaEventRecord( c.ev[ 1 ], s ) );
 		WSP_CHECK( encodeAsync( c, nullptr, batch ) );

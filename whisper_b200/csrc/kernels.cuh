@@ -37,8 +37,8 @@ namespace kern
 	};
 	// The phase vocoder (speed-up, whisper.cpp:2299-2311) takes a second MelTables of the same layout: hann [800] and twiddle [800] of the
 	// 800-point transform, cosT / sinT unset, filters and band shared with the 400-point tables.
-	// pcm [nSamples] -> raw log10 mel [80][nLen] (row = band) and the running maximum (ordered-int encoded float) in *maxSlot
-	// up to MEL_BATCH chunks transformed and normalised by one launch each (power, normalise); maxSlots[b] is chunk b's maximum
+	// up to MEL_BATCH chunks transformed and normalised by one launch each (power, normalise); single clips and streamed windows are
+	// a batch of one.  Chunk b: pcm [nSamples] -> log10 mel [80][nLen] (row = band), its maximum (ordered-int encoded float) in maxSlots[b]
 	constexpr int MEL_BATCH = 16;
 	struct MelBatch
 	{
@@ -49,11 +49,11 @@ namespace kern
 		int* maxSlots;                 // [count] consecutive
 		int count;
 	};
-	// speedUp: the phase vocoder (800-point transform, hop 320, tb = its tables) instead of the 400-point one (hop 160)
-	cudaError_t melBatch( const MelTables& tb, const MelBatch& mb, bool speedUp, cudaStream_t s );
-	cudaError_t melPower( const MelTables& tb, const float* pcm, int nSamples, int nLen, float* melRaw, int* maxSlot, bool speedUp, cudaStream_t s );
-	// in place: clamp to (max - 8), (x + 4) / 4
-	cudaError_t melNormalize( float* mel, int count, const int* maxSlot, cudaStream_t s );
+	// raw log10 mel and maxSlots; speedUp: the phase vocoder (800-point transform, hop 320, tb = its tables) instead of the 400-point
+	// one (hop 160)
+	cudaError_t melBatchPower( const MelTables& tb, const MelBatch& mb, bool speedUp, cudaStream_t s );
+	// in place: clamp to (maxSlots[b] - 8), (x + 4) / 4
+	cudaError_t melBatchNormalize( const MelBatch& mb, cudaStream_t s );
 	// mel f32 [80][nLen] at frame offset -> time-major f16 window [1 + frames + 1][80], halo rows (conv padding) written as zeros;
 	// frames = 2 * audio_ctx (3000 by default)
 	cudaError_t melWindow( const float* mel, int nLen, int offset, __half* dst, int frames, cudaStream_t s );

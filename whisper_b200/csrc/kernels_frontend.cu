@@ -129,13 +129,7 @@ namespace kern
 		}
 	}
 
-	template<int FFT>
-	__global__ void __launch_bounds__( MelGeom<FFT>::THREADS )
-		mel_power_kernel( MelTables tb, const float* __restrict__ pcm, int nSamples, int nLen, float* __restrict__ melRaw, int* maxSlot )
-	{
-		melFrame<FFT>( tb, pcm, nSamples, nLen, melRaw, maxSlot, blockIdx.x );
-	}
-	// the same for up to MEL_BATCH chunks in one launch: blockIdx.y = chunk (the driver loop of BASELINE.md §2 transforms B chunks per step)
+	// up to MEL_BATCH chunks in one launch: blockIdx.y = chunk (the driver loop of BASELINE.md §2 transforms B chunks per step)
 	template<int FFT>
 	__global__ void __launch_bounds__( MelGeom<FFT>::THREADS )
 		mel_power_batch_kernel( MelTables tb, MelBatch mb )
@@ -153,12 +147,6 @@ namespace kern
 		if( (double)v < mmax ) v = (float)mmax;
 		mel[ i ] = (float)( ( (double)v + 4.0 ) / 4.0 );
 	}
-	__global__ void mel_norm_kernel( float* mel, int count, const int* maxSlot )
-	{
-		const int i = blockIdx.x * blockDim.x + threadIdx.x;
-		if( i >= count ) return;
-		melNormOne( mel, i, maxSlot );
-	}
 	__global__ void mel_norm_batch_kernel( MelBatch mb )
 	{
 		const int b = blockIdx.y;
@@ -169,23 +157,18 @@ namespace kern
 
 	__global__ void init_max_kernel( int* maxSlot ) { maxSlot[ threadIdx.x ] = orderedFromFloat( -1e20f ); }
 
-	cudaError_t melPower( const MelTables& tb, const float* pcm, int nSamples, int nLen, float* melRaw, int* maxSlot, bool speedUp, cudaStream_t s )
+	// the longest chunk's frame count (the grid's x extent), or -1 for a batch size outside 1..MEL_BATCH
+	static int melBatchFrames( const MelBatch& mb )
 	{
-		init_max_kernel<<<1, 1, 0, s>>>( maxSlot );
-		if( nLen > 0 )
-		{
-			if( speedUp )
-				mel_power_kernel<800><<<nLen, MelGeom<800>::THREADS, 0, s>>>( tb, pcm, nSamples, nLen, melRaw, maxSlot );
-			else
-				mel_power_kernel<400><<<nLen, MelGeom<400>::THREADS, 0, s>>>( tb, pcm, nSamples, nLen, melRaw, maxSlot );
-		}
-		return cudaGetLastError();
-	}
-	cudaError_t melBatch( const MelTables& tb, const MelBatch& mb, bool speedUp, cudaStream_t s )
-	{
-		if( mb.count < 1 || mb.count > MEL_BATCH ) return cudaErrorInvalidValue;
+		if( mb.count < 1 || mb.count > MEL_BATCH ) return -1;
 		int maxLen = 0;
 		for( int b = 0; b < mb.count; b++ ) maxLen = mb.nLen[ b ] > maxLen ? mb.nLen[ b ] : maxLen;
+		return maxLen;
+	}
+	cudaError_t melBatchPower( const MelTables& tb, const MelBatch& mb, bool speedUp, cudaStream_t s )
+	{
+		const int maxLen = melBatchFrames( mb );
+		if( maxLen < 0 ) return cudaErrorInvalidValue;
 		init_max_kernel<<<1, mb.count, 0, s>>>( mb.maxSlots );
 		if( maxLen > 0 )
 		{
@@ -193,14 +176,15 @@ namespace kern
 				mel_power_batch_kernel<800><<<dim3( maxLen, mb.count ), MelGeom<800>::THREADS, 0, s>>>( tb, mb );
 			else
 				mel_power_batch_kernel<400><<<dim3( maxLen, mb.count ), MelGeom<400>::THREADS, 0, s>>>( tb, mb );
-			mel_norm_batch_kernel<<<dim3( ( MEL_BANDS * maxLen + 255 ) / 256, mb.count ), 256, 0, s>>>( mb );
 		}
 		return cudaGetLastError();
 	}
-	cudaError_t melNormalize( float* mel, int count, const int* maxSlot, cudaStream_t s )
+	cudaError_t melBatchNormalize( const MelBatch& mb, cudaStream_t s )
 	{
-		if( count > 0 )
-			mel_norm_kernel<<<( count + 255 ) / 256, 256, 0, s>>>( mel, count, maxSlot );
+		const int maxLen = melBatchFrames( mb );
+		if( maxLen < 0 ) return cudaErrorInvalidValue;
+		if( maxLen > 0 )
+			mel_norm_batch_kernel<<<dim3( ( MEL_BANDS * maxLen + 255 ) / 256, mb.count ), 256, 0, s>>>( mb );
 		return cudaGetLastError();
 	}
 

@@ -3,7 +3,7 @@
 //
 // Reference: Whisper/Whisper/MelStreamer.{h,cpp} + Whisper/MF/PcmReader.{h,cpp}.  There the queue holds 10 ms PCM chunks AND their
 // mel columns, computed on the CPU either on demand (MelStreamerSimple) or ahead of time by a background thread that keeps 2 x 3000
-// columns ready (MelStreamerThread, prebufferChunks).  Here a window's log-mel is a fraction of a millisecond of GPU time (mel_power_kernel), so only
+// columns ready (MelStreamerThread, prebufferChunks).  Here a window's log-mel is a fraction of a millisecond of GPU time (mel_power_batch_kernel), so only
 // the PCM is queued and the window is transformed when the loop asks for it; what the background thread buys is the SOURCE's
 // latency (file reads, decoding, a live feed), and it keeps the same 60 s ahead.  Semantics kept from the reference:
 //   * forward only: a window that starts before the previous one fails (MelStreamer.cpp:176-180 "doesn't support backwards seeks");
