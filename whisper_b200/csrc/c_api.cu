@@ -385,7 +385,6 @@ wsp_status wsp_set_reference_threads( wsp_context* c, int32_t n )
 {
 	if( !c ) return fail( WSP_E_POINTER, "context" );
 	if( n < 1 || n > kern::kMaxRefThreads ) return fail( WSP_E_INVALIDARG, "reference thread count must be in [1, 16]" );
-	if( n != c->c->refThreads && c->c->stepGraph ) { cudaGraphExecDestroy( c->c->stepGraph ); c->c->stepGraph = nullptr; }
 	c->c->refThreads = n;
 	return WSP_OK;
 }
@@ -401,14 +400,12 @@ wsp_status wsp_debug_set_step_mode( wsp_context* c, int32_t on )
 	if( !c ) return fail( WSP_E_POINTER, "context" );
 	// 0 = one kernel per op, 1 = round 1's barrier kernel, 2 = dataflow kernel (default)
 	if( on < 0 || on > 2 ) return fail( WSP_E_INVALIDARG, "step mode" );
-	if( on != c->c->stepMode && c->c->stepGraph ) { cudaGraphExecDestroy( c->c->stepGraph ); c->c->stepGraph = nullptr; }
 	c->c->stepMode = on;
 	return WSP_OK;
 }
 wsp_status wsp_debug_enable_step_timing( wsp_context* c, int32_t on )
 {
 	if( !c ) return fail( WSP_E_POINTER, "context" );
-	if( ( on != 0 ) != c->c->stepTiming && c->c->stepGraph ) { cudaGraphExecDestroy( c->c->stepGraph ); c->c->stepGraph = nullptr; }
 	c->c->stepTiming = on != 0;
 	return WSP_OK;
 }

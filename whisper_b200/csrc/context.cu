@@ -36,7 +36,7 @@ namespace wsp
 		for( auto& s : slots ) { if( s.mel ) cudaFree( s.mel ); if( s.pcm ) cudaFree( s.pcm ); }
 		for( auto& v : prof.pool ) cudaEventDestroy( v );
 		for( auto& v : timerEv ) if( v ) cudaEventDestroy( v );
-		void* bufs[] = { flowLayers, flowBias, flowExch, flowCtrl, megaLayers, megaBarrier, stepMarks, melMax, pcmDev, melF16, conv1, x, xn, q, k, vt, attn, h, crossK, crossV, selfK, selfV, xd, qd, attnD, hD, logits, probs, tieScratch,
+		void* bufs[] = { stepLayers, flowBias, flowExch, flowCtrl, megaBarrier, stepMarks, melMax, pcmDev, melF16, conv1, x, xn, q, k, vt, attn, h, crossK, crossV, selfK, selfV, xd, qd, attnD, hD, logits, probs, tieScratch,
 			tokensDev, dNPast, sampled, history };
 		for( void* b : bufs ) if( b ) cudaFree( b );
 		for( auto& v : ev ) if( v ) cudaEventDestroy( v );
@@ -121,37 +121,30 @@ namespace wsp
 		ok &= gemm::makeMap2D( &c.mapK, c.k, 64, B * H * T, 128, 128 );
 		ok &= gemm::makeMap2D( &c.mapVt, c.vt, c.Tp, B * H * 64, (uint64_t)c.Tp * 2, 64 );
 		if( !ok ) return fail( WSP_E_CUDA, "cuTensorMapEncodeTiled failed (driver too old for TMA?)" );
-		// per-layer pointer tables of the two decoder-step kernels: the persistent one (decode_mega.cu) and the dataflow one
+		// per-layer pointer table of the two decoder-step kernels: the persistent one (decode_mega.cu) and the dataflow one
 		// (decode_flow.cu, which also gets per-CTA bias slabs and sentinel-filled exchange buffers)
 		{
 			const kern::FlowGeom g = kern::flowGeometry( d, hp.n_vocab, e->numSMs );
 			c.flowGeom = g;
 			const size_t slabLayer = (size_t)g.grid * g.slabFloats;
 			WSP_CHECK( devAlloc( c.flowBias, slabLayer * L ) );
-			std::vector<kern::MegaLayer> ml( (size_t)L );
-			std::vector<kern::FlowLayer> fl( (size_t)L );
+			std::vector<kern::DecStepLayer> sl( (size_t)L );
 			for( int i = 0; i < L; i++ )
 			{
 				const DecLayerW& W = e->dec[ i ];
-				auto common = [ & ]( auto& m ) {
-					m.ln1g = W.ln1.g; m.ln1b = W.ln1.b; m.lncg = W.lnc.g; m.lncb = W.lnc.b; m.ln3g = W.ln3.g; m.ln3b = W.ln3.b;
-					m.wqkv = W.wqkv; m.wo = W.wo; m.wcq = W.wcq; m.wco = W.wco; m.w1 = W.w1; m.w2 = W.w2;
-					m.kCache = c.selfK + (size_t)i * B * hp.n_text_ctx * d;
-					m.vCache = c.selfV + (size_t)i * B * hp.n_text_ctx * d;
-					m.crossK = c.crossK + (size_t)i * B * T * d;
-					m.crossV = c.crossV + (size_t)i * B * T * d;
-				};
-				kern::MegaLayer& m = ml[ i ];
-				common( m );
+				kern::DecStepLayer& m = sl[ i ];
+				m.ln1g = W.ln1.g; m.ln1b = W.ln1.b; m.lncg = W.lnc.g; m.lncb = W.lnc.b; m.ln3g = W.ln3.g; m.ln3b = W.ln3.b;
+				m.wqkv = W.wqkv; m.wo = W.wo; m.wcq = W.wcq; m.wco = W.wco; m.w1 = W.w1; m.w2 = W.w2;
 				m.bqkv = W.bqkv; m.bo = W.bo; m.bcq = W.bcq; m.bco = W.bco; m.b1 = W.b1; m.b2 = W.b2;
-				common( fl[ i ] );
-				fl[ i ].biasSlab = c.flowBias + (size_t)i * slabLayer;
+				m.biasSlab = c.flowBias + (size_t)i * slabLayer;
+				m.kCache = c.selfK + (size_t)i * B * hp.n_text_ctx * d;
+				m.vCache = c.selfV + (size_t)i * B * hp.n_text_ctx * d;
+				m.crossK = c.crossK + (size_t)i * B * T * d;
+				m.crossV = c.crossV + (size_t)i * B * T * d;
 				WSP_CUDA( kern::flowBuildBiasSlab( c.flowBias + (size_t)i * slabLayer, g, d, W.bqkv, W.bo, W.bcq, W.bco, W.b1, W.b2, c.stream ) );
 			}
-			WSP_CHECK( devAlloc( c.megaLayers, (size_t)L ) );
-			WSP_CUDA( cudaMemcpy( c.megaLayers, ml.data(), ml.size() * sizeof( kern::MegaLayer ), cudaMemcpyHostToDevice ) );
-			WSP_CHECK( devAlloc( c.flowLayers, (size_t)L ) );
-			WSP_CUDA( cudaMemcpy( c.flowLayers, fl.data(), fl.size() * sizeof( kern::FlowLayer ), cudaMemcpyHostToDevice ) );
+			WSP_CHECK( devAlloc( c.stepLayers, (size_t)L ) );
+			WSP_CUDA( cudaMemcpy( c.stepLayers, sl.data(), sl.size() * sizeof( kern::DecStepLayer ), cudaMemcpyHostToDevice ) );
 			WSP_CHECK( devAlloc( c.megaBarrier, 64, true ) );
 			const size_t exBytes = kern::flowExchangeBytes( d, maxBatch, L );
 			WSP_CHECK( devAlloc( c.flowExch, exBytes ) );
@@ -168,6 +161,31 @@ namespace wsp
 		*out = cp.release();
 		return WSP_OK;
 	}
+
+	// ===============================================================================================================
+	// stage timing (wsp_timings): 0 = mel, 1 = encoder, 2 = decoder
+	// ===============================================================================================================
+	static float addStage( Context& c, int stage, cudaEvent_t from, cudaEvent_t to, int calls )
+	{
+		float ms = 0;
+		cudaEventElapsedTime( &ms, from, to );
+		c.ms[ stage ] += ms; c.calls[ stage ] += calls;
+		return ms;
+	}
+	// one call of a stage: what work() enqueues is timed, what after() enqueues (results on their way back) is not; returns synchronised
+	template<class W, class A>
+	static int timeStage( Context& c, int stage, W work, A after )
+	{
+		WSP_CUDA( cudaEventRecord( c.ev[ 0 ], c.stream ) );
+		WSP_CHECK( work() );
+		WSP_CUDA( cudaEventRecord( c.ev[ 1 ], c.stream ) );
+		WSP_CHECK( after() );
+		WSP_CUDA( cudaStreamSynchronize( c.stream ) );
+		addStage( c, stage, c.ev[ 0 ], c.ev[ 1 ], 1 );
+		return WSP_OK;
+	}
+	template<class W>
+	static int timeStage( Context& c, int stage, W work ) { return timeStage( c, stage, work, []() -> int { return WSP_OK; } ); }
 
 	// ===============================================================================================================
 	// mel
@@ -239,16 +257,11 @@ namespace wsp
 	{
 		WSP_CUDA( cudaSetDevice( c.e->device ) );
 		WSP_CHECK( ensurePcm( c, (size_t)( nSamples > 0 ? nSamples : 1 ) ) );
-		WSP_CUDA( cudaEventRecord( c.ev[ 0 ], c.stream ) );
-		if( nSamples > 0 )
-			WSP_CUDA( cudaMemcpyAsync( c.pcmDev, pcmHost, (size_t)nSamples * 4, cudaMemcpyHostToDevice, c.stream ) );
-		WSP_CHECK( melOf() );
-		WSP_CUDA( cudaEventRecord( c.ev[ 1 ], c.stream ) );
-		WSP_CUDA( cudaStreamSynchronize( c.stream ) );
-		float ms = 0;
-		cudaEventElapsedTime( &ms, c.ev[ 0 ], c.ev[ 1 ] );
-		c.ms[ 0 ] += ms; c.calls[ 0 ]++;
-		return WSP_OK;
+		return timeStage( c, 0, [ & ]() -> int {
+			if( nSamples > 0 )
+				WSP_CUDA( cudaMemcpyAsync( c.pcmDev, pcmHost, (size_t)nSamples * 4, cudaMemcpyHostToDevice, c.stream ) );
+			return melOf();
+		} );
 	}
 
 	int ctxPcmToMel( Context& c, int slot, const float* pcmHost, int nSamples )
@@ -420,14 +433,7 @@ namespace wsp
 	{
 		if( batch < 1 || batch > c.maxB ) return fail( WSP_E_BOUNDS, "batch exceeds the context's max_batch" );
 		WSP_CUDA( cudaSetDevice( c.e->device ) );
-		WSP_CUDA( cudaEventRecord( c.ev[ 0 ], c.stream ) );
-		WSP_CHECK( encodeAsync( c, offsets, batch ) );
-		WSP_CUDA( cudaEventRecord( c.ev[ 1 ], c.stream ) );
-		WSP_CUDA( cudaStreamSynchronize( c.stream ) );
-		float ms = 0;
-		cudaEventElapsedTime( &ms, c.ev[ 0 ], c.ev[ 1 ] );
-		c.ms[ 1 ] += ms; c.calls[ 1 ]++;
-		return WSP_OK;
+		return timeStage( c, 1, [ & ]() -> int { return encodeAsync( c, offsets, batch ); } );
 	}
 
 	// ===============================================================================================================
@@ -474,9 +480,8 @@ namespace wsp
 		return WSP_OK;
 	}
 
-	// Enqueue one decoder pass for `batch` chunks x N tokens.  Reads tokens from c.tokensDev, n_past / sampling flags from device
-	// scalars (so the N = 1 instance can be captured once as a CUDA graph and replayed for every step).
-	static int decodeEnqueue( Context& c, int N, int batch, bool allLogits, bool sample, int* launchesOut )
+	// One decoder pass kernel by kernel (kernels_decode.cu): embedding, 8 launches per layer, final LN + logits
+	static int enqueuePerOp( Context& c, int N, int batch, bool allLogits, int& n )
 	{
 		Engine& e = *c.e;
 		const HParams& hp = e.hp;
@@ -485,86 +490,83 @@ namespace wsp
 		cudaStream_t s = c.stream;
 		const int cols = batch * N;
 		const float qkScale = (float)pow( 64.0, -0.25 );   // whisper.cpp:1588, 1595, 1700
-		int n = 0;
-		if( N == 1 && !allLogits && c.stepMode == 2 && kern::flowSupported( d, batch, T, H, nCtx, c.refThreads, e.numSMs ) )
-		{
-			// steady state: ONE dataflow kernel for embedding + all layers + logits (decode_flow.cu), then the sampler
-			kern::FlowArgs fa;
-			fa.layers = c.flowLayers; fa.L = hp.n_text_layer; fa.B = batch; fa.maxB = c.maxB; fa.H = H; fa.nTextCtx = nCtx; fa.T = T; fa.nVocab = hp.n_vocab;
-			fa.refThreads = c.refThreads;
-			fa.tokEmb = e.tokEmb; fa.decPos = e.decPos; fa.lnfg = e.decLn.g; fa.lnfb = e.decLn.b;
-			fa.tokens = c.tokensDev; fa.dNPast = c.dNPast;
-			fa.exch = c.flowExch; fa.ctrl = c.flowCtrl; fa.logits = c.logits; fa.timing = c.stepTiming ? c.stepMarks : nullptr;
-			fa.g = c.flowGeom;
-			fa.timingCta = c.stepTimingCta;
-			WSP_KERNEL( KK_SKINNY, kern::decodeStepFlow( fa, d, e.numSMs, s ) ); n++;
-			if( sample ) { WSP_CHECK( enqueueSampler( c, N, batch ) ); n += 2; }
-			if( launchesOut ) *launchesOut = n;
-			return WSP_OK;
-		}
-		if( N == 1 && !allLogits && c.stepMode == 1 && kern::megaSupported( d, batch, T ) )
-		{
-			// steady state: one persistent kernel for embedding + all layers + logits (decode_mega.cu), then the sampler
-			kern::MegaArgs ma;
-			ma.layers = c.megaLayers; ma.L = hp.n_text_layer; ma.B = batch; ma.H = H; ma.nTextCtx = nCtx; ma.T = T; ma.nVocab = hp.n_vocab;
-			ma.refThreads = c.refThreads;
-			ma.tokEmb = e.tokEmb; ma.decPos = e.decPos; ma.lnfg = e.decLn.g; ma.lnfb = e.decLn.b;
-			ma.tokens = c.tokensDev; ma.dNPast = c.dNPast;
-			ma.x = c.xd; ma.q = c.qd; ma.attn = c.attnD; ma.h = c.hD; ma.logits = c.logits; ma.barrier = c.megaBarrier; ma.timing = c.stepTiming ? c.stepMarks : nullptr;
-			WSP_KERNEL( KK_SKINNY, kern::decodeStepMega( ma, d, e.numSMs, s ) ); n++;
-			if( sample ) { WSP_CHECK( enqueueSampler( c, N, batch ) ); n += 2; }
-			if( launchesOut ) *launchesOut = n;
-			return WSP_OK;
-		}
+		// y = epi( W x + bias ) for every column: x = LayerNorm( c.xd ) with `ln`, or the f16 rows xF16 when ln is null
+		auto skinny = [ & ]( const __half* W, const float* bias, int nOut, int K, const LnW* ln, const __half* xF16, kern::SkinnyEpi epi, float* outF32, __half* outF16 = nullptr ) {
+			kern::SkinnyArgs a;
+			a.W = W; a.nOut = nOut; a.K = K; a.xStride = K; a.nCols = cols;
+			if( ln ) { a.xF32 = c.xd; a.gamma = ln->g; a.beta = ln->b; }
+			else a.xF16 = xF16;
+			a.epi = epi; a.bias = bias; a.outF32 = outF32; a.outF16 = outF16;
+			if( epi == kern::SK_QKV || epi == kern::SK_Q_SCALE ) a.scale = qkScale;
+			a.ld = epi == kern::SK_QKV ? d : nOut;
+			return a;
+		};
 		WSP_KERNEL( KK_OTHER, kern::embedTokens( e.tokEmb, e.decPos, c.tokensDev, c.dNPast, c.xd, batch, N, d, s ) ); n++;
 		for( int il = 0; il < hp.n_text_layer; il++ )
 		{
 			const DecLayerW& W = e.dec[ il ];
 			__half* kc = c.selfK + (size_t)il * c.maxB * nCtx * d;
 			__half* vc = c.selfV + (size_t)il * c.maxB * nCtx * d;
-			kern::SkinnyArgs a;
 			// LN + (Q | K | V); K, V appended to the f16 self-KV cache in the epilogue (a14)
-			a = kern::SkinnyArgs();
-			a.W = W.wqkv; a.nOut = 3 * d; a.K = d; a.xF32 = c.xd; a.xStride = d; a.gamma = W.ln1.g; a.beta = W.ln1.b; a.nCols = cols;
-			a.epi = kern::SK_QKV; a.bias = W.bqkv; a.scale = qkScale; a.outF32 = c.qd; a.ld = d; a.kCache = kc; a.vCache = vc;
-			a.d = d; a.N = N; a.nTextCtx = nCtx; a.dNPast = c.dNPast;
+			kern::SkinnyArgs a = skinny( W.wqkv, W.bqkv, 3 * d, d, &W.ln1, nullptr, kern::SK_QKV, c.qd );
+			a.kCache = kc; a.vCache = vc; a.d = d; a.N = N; a.nTextCtx = nCtx; a.dNPast = c.dNPast;
 			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( a, s ) );
 			WSP_KERNEL( KK_SELF, kern::selfAttnDecode( c.qd, kc, vc, c.attnD, batch, N, H, d, nCtx, c.dNPast, c.refThreads, s ) );
-			a = kern::SkinnyArgs();
-			a.W = W.wo; a.nOut = d; a.K = d; a.xF16 = c.attnD; a.xStride = d; a.nCols = cols;
-			a.epi = kern::SK_BIAS_RESID; a.bias = W.bo; a.outF32 = c.xd; a.ld = d;
-			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( a, s ) );
+			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.wo, W.bo, d, d, nullptr, c.attnD, kern::SK_BIAS_RESID, c.xd ), s ) );
 			// cross attention (a15)
-			a = kern::SkinnyArgs();
-			a.W = W.wcq; a.nOut = d; a.K = d; a.xF32 = c.xd; a.xStride = d; a.gamma = W.lnc.g; a.beta = W.lnc.b; a.nCols = cols;
-			a.epi = kern::SK_Q_SCALE; a.bias = W.bcq; a.scale = qkScale; a.outF32 = c.qd; a.ld = d;
-			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( a, s ) );
+			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.wcq, W.bcq, d, d, &W.lnc, nullptr, kern::SK_Q_SCALE, c.qd ), s ) );
 			const size_t crossOff = (size_t)il * c.maxB * hp.n_audio_ctx * d;   // layer stride of the pointer tables, whatever T is
 			WSP_KERNEL( KK_CROSS, kern::crossAttnDecode( c.qd, c.crossK + crossOff, c.crossV + crossOff, c.attnD, batch, N, H, d, T, c.refThreads, s ) );
-			a = kern::SkinnyArgs();
-			a.W = W.wco; a.nOut = d; a.K = d; a.xF16 = c.attnD; a.xStride = d; a.nCols = cols;
-			a.epi = kern::SK_BIAS_RESID; a.bias = W.bco; a.outF32 = c.xd; a.ld = d;
-			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( a, s ) );
+			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.wco, W.bco, d, d, nullptr, c.attnD, kern::SK_BIAS_RESID, c.xd ), s ) );
 			// MLP (a16)
-			a = kern::SkinnyArgs();
-			a.W = W.w1; a.nOut = 4 * d; a.K = d; a.xF32 = c.xd; a.xStride = d; a.gamma = W.ln3.g; a.beta = W.ln3.b; a.nCols = cols;
-			a.epi = kern::SK_GELU_F16; a.bias = W.b1; a.outF16 = c.hD; a.ld = 4 * d;
-			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( a, s ) );
-			a = kern::SkinnyArgs();
-			a.W = W.w2; a.nOut = d; a.K = 4 * d; a.xF16 = c.hD; a.xStride = 4 * d; a.nCols = cols;
-			a.epi = kern::SK_BIAS_RESID; a.bias = W.b2; a.outF32 = c.xd; a.ld = d;
-			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( a, s ) );
+			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.w1, W.b1, 4 * d, d, &W.ln3, nullptr, kern::SK_GELU_F16, nullptr, c.hD ), s ) );
+			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.w2, W.b2, d, 4 * d, nullptr, c.hD, kern::SK_BIAS_RESID, c.xd ), s ) );
 			n += 8;
 		}
 		// final LN + logits = tok_emb^T x (a17): only the last token of each chunk unless all logits were requested
+		kern::SkinnyArgs a = skinny( e.tokEmb, nullptr, hp.n_vocab, d, &e.decLn, nullptr, kern::SK_LOGITS, c.logits );
+		if( !allLogits ) { a.xF32 = c.xd + (size_t)( N - 1 ) * d; a.xStride = (int64_t)N * d; a.nCols = batch; }
+		WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( a, s ) ); n++;
+		return WSP_OK;
+	}
+
+	// what both step kernels are handed alike
+	static kern::DecStepArgs stepArgs( const Context& c, int batch )
+	{
+		const Engine& e = *c.e;
+		const HParams& hp = e.hp;
+		kern::DecStepArgs a;
+		a.layers = c.stepLayers; a.L = hp.n_text_layer; a.B = batch; a.maxB = c.maxB; a.H = hp.n_text_head; a.nTextCtx = hp.n_text_ctx;
+		a.T = c.encCtx;   // cross-attention keys: the audio positions of the last encode (whisper.cpp:1528)
+		a.nVocab = hp.n_vocab; a.refThreads = c.refThreads;
+		a.tokEmb = e.tokEmb; a.decPos = e.decPos; a.lnfg = e.decLn.g; a.lnfb = e.decLn.b;
+		a.tokens = c.tokensDev; a.dNPast = c.dNPast; a.logits = c.logits; a.timing = c.stepTiming ? c.stepMarks : nullptr;
+		return a;
+	}
+
+	// Enqueue one decoder pass for `batch` chunks x N tokens.  Reads tokens from c.tokensDev, n_past / sampling flags from device
+	// scalars (so the N = 1 instance can be captured once as a CUDA graph and replayed for every step).
+	static int decodeEnqueue( Context& c, int N, int batch, bool allLogits, bool sample, int* launchesOut )
+	{
+		const Engine& e = *c.e;
+		const int d = e.hp.n_text_state;
+		const bool step = N == 1 && !allLogits;   // the steady state: embedding + all layers + logits in ONE kernel
+		const kern::DecStepArgs sa = stepArgs( c, batch );
+		int n = 0;
+		if( step && c.stepMode == 2 && kern::flowSupported( d, batch, sa.T, sa.H, sa.nTextCtx, c.refThreads, c.flowGeom ) )
 		{
-			kern::SkinnyArgs a;
-			a.W = e.tokEmb; a.nOut = hp.n_vocab; a.K = d; a.gamma = e.decLn.g; a.beta = e.decLn.b;
-			if( allLogits ) { a.xF32 = c.xd; a.xStride = d; a.nCols = cols; }
-			else { a.xF32 = c.xd + (size_t)( N - 1 ) * d; a.xStride = (int64_t)N * d; a.nCols = batch; }
-			a.epi = kern::SK_LOGITS; a.outF32 = c.logits; a.ld = hp.n_vocab;
-			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( a, s ) ); n++;
+			kern::FlowArgs fa{ sa };   // the dataflow kernel (decode_flow.cu)
+			fa.exch = c.flowExch; fa.ctrl = c.flowCtrl; fa.g = c.flowGeom; fa.timingCta = c.stepTimingCta;
+			WSP_KERNEL( KK_SKINNY, kern::decodeStepFlow( fa, d, e.numSMs, c.stream ) ); n++;
 		}
+		else if( step && c.stepMode == 1 && kern::megaSupported( d, batch, sa.T ) )
+		{
+			kern::MegaArgs ma{ sa };   // the persistent barrier kernel (decode_mega.cu)
+			ma.x = c.xd; ma.q = c.qd; ma.attn = c.attnD; ma.h = c.hD; ma.barrier = c.megaBarrier;
+			WSP_KERNEL( KK_SKINNY, kern::decodeStepMega( ma, d, e.numSMs, c.stream ) ); n++;
+		}
+		else
+			WSP_CHECK( enqueuePerOp( c, N, batch, allLogits, n ) );
 		if( sample && !allLogits ) { WSP_CHECK( enqueueSampler( c, N, batch ) ); n += 2; }
 		if( launchesOut ) *launchesOut = n;
 		return WSP_OK;
@@ -576,7 +578,8 @@ namespace wsp
 		int n = 0;
 		if( N == 1 && !allLogits && sample && c.useGraph && !c.prof.on )
 		{
-			if( !c.stepGraph || c.stepGraphBatch != batch || c.stepGraphCtx != c.encCtx )
+			const StepGraphKey key{ batch, c.encCtx, c.refThreads, c.stepMode, c.stepTiming };
+			if( !c.stepGraph || !( c.stepGraphKey == key ) )
 			{
 				if( c.stepGraph ) { cudaGraphExecDestroy( c.stepGraph ); c.stepGraph = nullptr; }
 				cudaGraph_t graph = nullptr;
@@ -588,8 +591,7 @@ namespace wsp
 				ce = cudaGraphInstantiate( &c.stepGraph, graph, 0 );
 				cudaGraphDestroy( graph );
 				WSP_CUDA( ce );
-				c.stepGraphBatch = batch;
-				c.stepGraphCtx = c.encCtx;
+				c.stepGraphKey = key;
 				c.stepGraphLaunches = n;
 			}
 			WSP_CUDA( cudaGraphLaunch( c.stepGraph, c.stream ) );
@@ -621,31 +623,30 @@ namespace wsp
 		if( !devTokens && ( nPast < 0 || nPast + nTokens > hp.n_text_ctx ) ) return fail( WSP_E_BOUNDS, "n_past + n_tokens exceeds n_text_ctx" );
 		// device-fed tokens continue from the device's n_past: its host mirror guards the KV cache and the positional table
 		if( devTokens && c.nPastHost + nTokens > hp.n_text_ctx ) return fail( WSP_E_BOUNDS, "n_past + n_tokens exceeds n_text_ctx" );
-		WSP_CUDA( cudaSetDevice( c.e->device ) );
-		cudaStream_t s = c.stream;
-		WSP_CUDA( cudaEventRecord( c.ev[ 0 ], s ) );
 		if( !devTokens )
-		{
 			for( int i = 0; i < batch * nTokens; i++ )
 				if( tokensHost[ i ] < 0 || tokensHost[ i ] >= hp.n_vocab ) return fail( WSP_E_INVALIDARG, "token id out of range" );
-			WSP_CUDA( cudaMemcpyAsync( c.tokensDev, tokensHost, (size_t)batch * nTokens * 4, cudaMemcpyHostToDevice, s ) );
-			WSP_CUDA( kern::setInts( c.dNPast, nPast, 0, s ) );
-			WSP_CUDA( kern::setInts( c.dFlags, ( flags & WSP_DECODE_FORCE_TIMESTAMP ) ? 1 : 0, ( flags & WSP_DECODE_INITIAL ) ? 1 : 0, s ) );
-			launched( 2 );
-		}
-		WSP_CHECK( decodeSubmit( c, nTokens, batch, allLogits, sample ) );
-		// the device advances n_past only when it samples (advance_kernel): mirror exactly that
-		if( !devTokens ) c.nPastHost = nPast;
-		if( sample && !allLogits ) c.nPastHost += nTokens;
-		c.lastLogitRows = allLogits ? batch * nTokens : batch;
-		WSP_CUDA( cudaEventRecord( c.ev[ 1 ], s ) );
-		if( sampledHost && sample && !allLogits )
-			WSP_CUDA( cudaMemcpyAsync( sampledHost, c.sampled, (size_t)batch * sizeof( wsp_token_data ), cudaMemcpyDeviceToHost, s ) );
-		WSP_CUDA( cudaStreamSynchronize( s ) );
-		float ms = 0;
-		cudaEventElapsedTime( &ms, c.ev[ 0 ], c.ev[ 1 ] );
-		c.ms[ 2 ] += ms; c.calls[ 2 ]++;
-		return WSP_OK;
+		WSP_CUDA( cudaSetDevice( c.e->device ) );
+		cudaStream_t s = c.stream;
+		return timeStage( c, 2, [ & ]() -> int {
+			if( !devTokens )
+			{
+				WSP_CUDA( cudaMemcpyAsync( c.tokensDev, tokensHost, (size_t)batch * nTokens * 4, cudaMemcpyHostToDevice, s ) );
+				WSP_CUDA( kern::setInts( c.dNPast, nPast, 0, s ) );
+				WSP_CUDA( kern::setInts( c.dFlags, ( flags & WSP_DECODE_FORCE_TIMESTAMP ) ? 1 : 0, ( flags & WSP_DECODE_INITIAL ) ? 1 : 0, s ) );
+				launched( 2 );
+			}
+			WSP_CHECK( decodeSubmit( c, nTokens, batch, allLogits, sample ) );
+			// the device advances n_past only when it samples (advance_kernel): mirror exactly that
+			if( !devTokens ) c.nPastHost = nPast;
+			if( sample && !allLogits ) c.nPastHost += nTokens;
+			c.lastLogitRows = allLogits ? batch * nTokens : batch;
+			return WSP_OK;
+		}, [ & ]() -> int {
+			if( sampledHost && sample && !allLogits )
+				WSP_CUDA( cudaMemcpyAsync( sampledHost, c.sampled, (size_t)batch * sizeof( wsp_token_data ), cudaMemcpyDeviceToHost, s ) );
+			return WSP_OK;
+		} );
 	}
 
 	int ctxUploadPcm( Context& c, int slot, const float* pcmHost, int nSamples )
@@ -753,11 +754,9 @@ namespace wsp
 		if( tokensOut )
 			for( int b = 0; b < batch; b++ )
 				for( int i = 0; i < nDecode; i++ ) tokensOut[ (size_t)b * nDecode + i ] = hist[ (size_t)b * c.histCap + i ];
-		float m0 = 0, m1 = 0, m2 = 0;
-		cudaEventElapsedTime( &m0, c.ev[ 0 ], c.ev[ 1 ] );
-		cudaEventElapsedTime( &m1, c.ev[ 1 ], c.ev[ 2 ] );
-		cudaEventElapsedTime( &m2, c.ev[ 2 ], c.ev[ 3 ] );
-		c.ms[ 0 ] += m0; c.ms[ 1 ] += m1; c.ms[ 2 ] += m2; c.calls[ 0 ]++; c.calls[ 1 ]++; c.calls[ 2 ] += nDecode;
+		const float m0 = addStage( c, 0, c.ev[ 0 ], c.ev[ 1 ], 1 );
+		const float m1 = addStage( c, 1, c.ev[ 1 ], c.ev[ 2 ], 1 );
+		const float m2 = addStage( c, 2, c.ev[ 2 ], c.ev[ 3 ], nDecode );
 		if( stageMs ) { stageMs[ 0 ] = m0; stageMs[ 1 ] = m1; stageMs[ 2 ] = m2; }
 		return WSP_OK;
 	}

@@ -23,6 +23,7 @@
 #include "ptx.cuh"
 #include "ref_arith.cuh"
 #include <math.h>
+#include <type_traits>
 
 namespace kern
 {
@@ -612,7 +613,7 @@ namespace kern
 				};
 				for( int il = 0; il < L; il++ )
 				{
-					const FlowLayer& Lr = a.layers[ il ];
+					const DecStepLayer& Lr = a.layers[ il ];
 					sendParams( Lr.ln1g, Lr.ln1b, Lr.biasSlab + (size_t)cta * g.slabFloats, g.slabFloats );
 					sendWeights( Lr.wqkv, D, r3, n3, 1 );
 					for( int unit = cta; unit < B * H; unit += G )
@@ -713,7 +714,7 @@ namespace kern
 			for( int il = 0; il <= L; il++ )
 			{
 				const bool last = il == L;                // final LayerNorm + logits (a17)
-				const FlowLayer& Lr = a.layers[ last ? L - 1 : il ];
+				const DecStepLayer& Lr = a.layers[ last ? L - 1 : il ];
 				uint8_t* const exb = a.exch + ( (size_t)set * L + ( last ? L - 1 : il ) ) * exLayer;
 				float* const x1 = reinterpret_cast<float*>( exb );
 				float* const x2 = x1 + colsD;
@@ -1145,6 +1146,22 @@ namespace kern
 			return cudaLaunchKernelEx( &cfg, decode_flow_kernel<D, false>, (const FlowArgs)a );
 		}
 		inline int pad4( int x ) { return ( x + 3 ) & ~3; }
+
+		// the decoder widths the kernel is instantiated for: f( integral_constant<int, D> ) for d == D, `unsupported` for any other d
+		template<class R, class F>
+		R dispatchD( int d, R unsupported, F&& f )
+		{
+			switch( d )
+			{
+			case 128: return f( std::integral_constant<int, 128>() );
+			case 384: return f( std::integral_constant<int, 384>() );
+			case 512: return f( std::integral_constant<int, 512>() );
+			case 768: return f( std::integral_constant<int, 768>() );
+			case 1024: return f( std::integral_constant<int, 1024>() );
+			case 1280: return f( std::integral_constant<int, 1280>() );
+			default: return unsupported;
+			}
+		}
 	}
 
 	FlowGeom flowGeometry( int d, int nVocab, int grid )
@@ -1165,36 +1182,20 @@ namespace kern
 		return g;
 	}
 
-	bool flowSupported( int d, int B, int T, int H, int nTextCtx, int refThreads, int grid )
+	bool flowSupported( int d, int B, int T, int H, int nTextCtx, int refThreads, const FlowGeom& g )
 	{
 		if( B < 1 || B > 16 || T > FL_MAXT || T < 1 || H * 64 != d || nTextCtx > FL_MAXT ) return false;
 		if( refThreads < 1 || refThreads > kMaxRefThreads ) return false;
-		if( !( d == 128 || d == 384 || d == 512 || d == 768 || d == 1024 || d == 1280 ) ) return false;
-		const FlowGeom g = flowGeometry( d, 51865, grid );
 		if( g.R1 > 16 || g.slabFloats > 256 ) return false;
-		const int rs = 2 * d + 64;
-		const int slot = 8 * rs > 16384 ? 8 * rs : 16384;
-		const int cr = ( slot / 128 ) & ~7;
-		const int ns = ringSlots( slot, rs, B > 8 ? 16 : 8 );
-		(void)cr;
-		if( 4 + 1 > ns ) return false;   // a round of V slots (one per reference thread) is held at once
-		return true;
+		const int ns = dispatchD( d, 0, [ & ]( auto D ) { int n = 0; smemBytes<decltype( D )::value>( B > 8 ? 16 : 8, n ); return n; } );
+		return ns >= 4 + 1;   // a round of V slots (one per reference thread) is held at once
 	}
 
 	size_t flowExchangeBytes( int d, int maxB, int L ) { return (size_t)2 * L * maxB * d * 32; }
 
 	cudaError_t flowPrepare( int d )
 	{
-		switch( d )
-		{
-		case 128: return prepareD<128>();
-		case 384: return prepareD<384>();
-		case 512: return prepareD<512>();
-		case 768: return prepareD<768>();
-		case 1024: return prepareD<1024>();
-		case 1280: return prepareD<1280>();
-		default: return cudaSuccess;
-		}
+		return dispatchD( d, cudaSuccess, []( auto D ) { return prepareD<decltype( D )::value>(); } );
 	}
 
 	cudaError_t flowBuildBiasSlab( float* slab, const FlowGeom& g, int d, const float* bqkv, const float* bo, const float* bcq, const float* bco,
@@ -1206,15 +1207,6 @@ namespace kern
 
 	cudaError_t decodeStepFlow( FlowArgs a, int d, int numSMs, cudaStream_t s )
 	{
-		switch( d )
-		{
-		case 128: return launchD<128>( a, numSMs, s );
-		case 384: return launchD<384>( a, numSMs, s );
-		case 512: return launchD<512>( a, numSMs, s );
-		case 768: return launchD<768>( a, numSMs, s );
-		case 1024: return launchD<1024>( a, numSMs, s );
-		case 1280: return launchD<1280>( a, numSMs, s );
-		default: return cudaErrorInvalidValue;
-		}
+		return dispatchD( d, cudaErrorInvalidValue, [ & ]( auto D ) { return launchD<decltype( D )::value>( a, numSMs, s ); } );
 	}
 }

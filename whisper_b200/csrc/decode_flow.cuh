@@ -1,19 +1,9 @@
 // Dataflow decoder-step kernel — see decode_flow.cu.
 #pragma once
-#include <cuda_fp16.h>
-#include <cuda_runtime.h>
-#include <stdint.h>
+#include "decode_step.cuh"
 
 namespace kern
 {
-	struct FlowLayer
-	{
-		const float *ln1g, *ln1b, *lncg, *lncb, *ln3g, *ln3b;
-		const __half *wqkv, *wo, *wcq, *wco, *w1, *w2;
-		const float* biasSlab;              // [grid][slabFloats]: this layer's biases regrouped per CTA (flowBuildBiasSlab)
-		__half *kCache, *vCache;            // [maxB][H][nTextCtx][64] of this layer (head-major: a head's rows are contiguous)
-		const __half *crossK, *crossV;      // [maxB][H][T][64] of this layer
-	};
 	// how the output rows of every weight-streaming phase are split over the CTAs: CTA c owns rows [c*R, min((c+1)*R, nOut))
 	struct FlowGeom
 	{
@@ -24,26 +14,17 @@ namespace kern
 	};
 	FlowGeom flowGeometry( int d, int nVocab, int grid );
 
-	struct FlowArgs
+	struct FlowArgs : DecStepArgs       // timing: (id, %globaltimer) marks of CTA `timingCta`
 	{
-		const FlowLayer* layers = nullptr;  // device array [L]
-		int L = 0, B = 0, maxB = 0, H = 0, nTextCtx = 0, T = 0, nVocab = 0, refThreads = 4;
-		const __half* tokEmb = nullptr;
-		const float* decPos = nullptr;
-		const float* lnfg = nullptr;
-		const float* lnfb = nullptr;
-		const int* tokens = nullptr;        // [B] (device)
-		const int* dNPast = nullptr;
 		uint8_t* exch = nullptr;            // exchange buffers: 2 sets x L layers x (maxB * d * 32) bytes, all 0xFF when idle
 		unsigned* ctrl = nullptr;           // [0] CTAs finished, [1] launch epoch (selects the exchange set)
-		float* logits = nullptr;            // [B][nVocab]
-		unsigned long long* timing = nullptr;   // optional: (id, %globaltimer) marks of CTA `timingCta` (debug)
 		int timingCta = 0;
 		FlowGeom g;
 		int NS = 0;                         // ring slots
 		int ncols = 8;                      // activation columns staged: 8 (B <= 8) or 16
 	};
-	bool flowSupported( int d, int B, int T, int H, int nTextCtx, int refThreads, int grid );
+	// g: the context's geometry (flowGeometry); the limits checked on it do not depend on the vocabulary, so neither does the answer
+	bool flowSupported( int d, int B, int T, int H, int nTextCtx, int refThreads, const FlowGeom& g );
 	size_t flowExchangeBytes( int d, int maxB, int L );
 	cudaError_t flowPrepare( int d );   // function attributes for the current device, outside any stream capture
 	// regroup one layer's biases per CTA: slab[c] = (qkv rows of c | o | cq | co | fc1 | fc2), zero padded

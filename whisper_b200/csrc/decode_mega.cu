@@ -14,6 +14,7 @@
 #include "ptx.cuh"
 #include "ref_arith.cuh"
 #include <math.h>
+#include <type_traits>
 
 namespace kern
 {
@@ -390,7 +391,7 @@ namespace kern
 		// copied to shared memory by cp.async BEFORE the barrier that publishes this step's new row; after it only 2 x 128 bytes remain.
 		constexpr int SA_KSTRIDE = 144;   // bytes per K row in smem (128 + 16: conflict-free 16-byte reads of one row per thread)
 		constexpr int SA_MAXKV = 448;
-		__device__ __forceinline__ void selfLoadRows( const MegaArgs& a, const MegaLayer& L, int d, const Smem& sm, int unit, int j0, int j1, int tid )
+		__device__ __forceinline__ void selfLoadRows( const MegaArgs& a, const DecStepLayer& L, int d, const Smem& sm, int unit, int j0, int j1, int tid )
 		{
 			if( unit >= a.B * a.H ) return;
 			const int b = unit / a.H, h = unit - b * a.H;
@@ -408,7 +409,7 @@ namespace kern
 				else ptx::cp_async16( sK + j * SA_KSTRIDE + c * 16, kb + (size_t)j * 64 + c * 8 );
 			}
 		}
-		__device__ void selfAttnPhase( const MegaArgs& a, const MegaLayer& L, int d, int nPast, const Smem& sm, int warp, int lane, int tid )
+		__device__ void selfAttnPhase( const MegaArgs& a, const DecStepLayer& L, int d, int nPast, const Smem& sm, int warp, int lane, int tid )
 		{
 			const int H = a.H;
 			const int nkv = min( nPast + 1, a.nTextCtx );
@@ -462,7 +463,7 @@ namespace kern
 			uint4 u[ kKBatch ];
 			int unit;
 		};
-		__device__ __forceinline__ void crossPrefetch( const MegaArgs& a, const MegaLayer& L, CrossPrefetch& pf, const Smem& sm, int unit, int warp, int lane, int tid )
+		__device__ __forceinline__ void crossPrefetch( const MegaArgs& a, const DecStepLayer& L, CrossPrefetch& pf, const Smem& sm, int unit, int warp, int lane, int tid )
 		{
 			pf.unit = unit;
 			if( unit >= a.B * a.H ) return;
@@ -474,7 +475,7 @@ namespace kern
 			ptx::cp_async_commit();
 			kStreamPrefetch( pf.u, reinterpret_cast<const uint4*>( L.crossK + base ), T, warp, lane );
 		}
-		__device__ void crossAttnPhase( const MegaArgs& a, const MegaLayer& L, int d, CrossPrefetch& pf, const Smem& sm, int warp, int lane, int tid )
+		__device__ void crossAttnPhase( const MegaArgs& a, const DecStepLayer& L, int d, CrossPrefetch& pf, const Smem& sm, int warp, int lane, int tid )
 		{
 			const int T = a.T, H = a.H;
 			float* sred = sm.misc + 64;
@@ -552,7 +553,7 @@ namespace kern
 					o.epi = EP_LOGITS; o.outF32 = a.logits; o.ld = a.nVocab;
 					return o;
 				}
-				const MegaLayer& L = a.layers[ il ];
+				const DecStepLayer& L = a.layers[ il ];
 				switch( ph )
 				{
 				case PH_QKV:   // LN1 + (Q | K | V), K/V appended to the cache (a14)
@@ -590,7 +591,7 @@ namespace kern
 
 			// a layer's cross-attention K/V tile of "my" (chunk, head) starts moving HBM -> L2 several phases ahead of its use (those
 			// phases are latency-bound and leave the DRAM pipe idle); issued while waiting at a barrier, off the critical path
-			auto crossL2 = [ & ]( const MegaLayer& L ) {
+			auto crossL2 = [ & ]( const DecStepLayer& L ) {
 				if( (int)blockIdx.x < B * a.H )
 				{
 					const size_t cb = (size_t)blockIdx.x * a.T * 64;
@@ -620,7 +621,7 @@ namespace kern
 #pragma unroll 1
 			for( int il = 0; il <= a.L; il++ )
 			{
-				const MegaLayer& L = a.layers[ il < a.L ? il : a.L - 1 ];
+				const DecStepLayer& L = a.layers[ il < a.L ? il : a.L - 1 ];
 #pragma unroll 1
 				for( int ph = 0; ph < PH_COUNT; ph++ )
 				{
@@ -716,39 +717,37 @@ namespace kern
 			decode_step_kernel<D><<<numSMs, MG_THREADS, SMEM, s>>>( a );
 			return cudaGetLastError();
 		}
+
+		// the decoder widths the kernel is instantiated for: f( integral_constant<int, D> ) for d == D, `unsupported` for any other d
+		template<class R, class F>
+		R dispatchD( int d, R unsupported, F&& f )
+		{
+			switch( d )
+			{
+			case 128: return f( std::integral_constant<int, 128>() );
+			case 384: return f( std::integral_constant<int, 384>() );
+			case 512: return f( std::integral_constant<int, 512>() );
+			case 768: return f( std::integral_constant<int, 768>() );
+			case 1024: return f( std::integral_constant<int, 1024>() );
+			case 1280: return f( std::integral_constant<int, 1280>() );
+			default: return unsupported;
+			}
+		}
 	}
 
 	bool megaSupported( int d, int B, int T )
 	{
 		if( B < 1 || B > 16 || T * 128 > MG_SMEM_A ) return false;
-		return d == 128 || d == 384 || d == 512 || d == 768 || d == 1024 || d == 1280;
+		return dispatchD( d, false, []( auto ) { return true; } );
 	}
 
 	cudaError_t megaPrepare( int d )
 	{
-		switch( d )
-		{
-		case 128: return prepareD<128>();
-		case 384: return prepareD<384>();
-		case 512: return prepareD<512>();
-		case 768: return prepareD<768>();
-		case 1024: return prepareD<1024>();
-		case 1280: return prepareD<1280>();
-		default: return cudaSuccess;
-		}
+		return dispatchD( d, cudaSuccess, []( auto D ) { return prepareD<decltype( D )::value>(); } );
 	}
 
 	cudaError_t decodeStepMega( const MegaArgs& a, int d, int numSMs, cudaStream_t s )
 	{
-		switch( d )
-		{
-		case 128: return launchD<128>( a, numSMs, s );
-		case 384: return launchD<384>( a, numSMs, s );
-		case 512: return launchD<512>( a, numSMs, s );
-		case 768: return launchD<768>( a, numSMs, s );
-		case 1024: return launchD<1024>( a, numSMs, s );
-		case 1280: return launchD<1280>( a, numSMs, s );
-		default: return cudaErrorInvalidValue;
-		}
+		return dispatchD( d, cudaErrorInvalidValue, [ & ]( auto D ) { return launchD<decltype( D )::value>( a, numSMs, s ); } );
 	}
 }

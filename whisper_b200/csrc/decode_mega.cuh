@@ -1,36 +1,16 @@
 // Persistent decoder-step kernel — see decode_mega.cu.
 #pragma once
-#include <cuda_fp16.h>
-#include <cuda_runtime.h>
-#include <stdint.h>
+#include "decode_step.cuh"
 
 namespace kern
 {
-	struct MegaLayer
+	struct MegaArgs : DecStepArgs       // timing: marks of CTA 0 around every barrier
 	{
-		const float *ln1g, *ln1b, *lncg, *lncb, *ln3g, *ln3b;
-		const __half *wqkv, *wo, *wcq, *wco, *w1, *w2;
-		const float *bqkv, *bo, *bcq, *bco, *b1, *b2;
-		__half *kCache, *vCache;            // [maxB][H][nTextCtx][64] of this layer (head-major)
-		const __half *crossK, *crossV;      // [maxB][H][T][64] of this layer
-	};
-	struct MegaArgs
-	{
-		const MegaLayer* layers = nullptr;  // device array [L]
-		int L = 0, B = 0, H = 0, nTextCtx = 0, T = 0, nVocab = 0, refThreads = 4;
-		const __half* tokEmb = nullptr;
-		const float* decPos = nullptr;
-		const float* lnfg = nullptr;
-		const float* lnfb = nullptr;
-		const int* tokens = nullptr;        // [B] (device)
-		const int* dNPast = nullptr;
 		float* x = nullptr;                 // [B][d] residual stream
 		float* q = nullptr;                 // [B][d]
 		__half* attn = nullptr;             // [B][d]
 		__half* h = nullptr;                // [B][4d]
-		float* logits = nullptr;            // [B][nVocab]
 		unsigned* barrier = nullptr;        // grid barrier counter (zeroed by the launcher)
-		unsigned long long* timing = nullptr;   // optional: %globaltimer marks of CTA 0 around every barrier (debug)
 	};
 	bool megaSupported( int d, int B, int T );
 	cudaError_t megaPrepare( int d );   // function attributes, outside any stream capture

@@ -107,6 +107,18 @@ namespace wsp
 		size_t used = 0;
 	};
 
+	// What a captured N = 1 step graph depends on.  The launches in it took their arguments by value at capture time, so every
+	// Context field that decodeEnqueue reads by value for the N = 1 path is a member: decodeSubmit re-captures when the key differs.
+	struct StepGraphKey
+	{
+		int batch = 0, encCtx = 0, refThreads = 0, stepMode = 0;
+		bool timing = false;
+		bool operator==( const StepGraphKey& o ) const
+		{
+			return batch == o.batch && encCtx == o.encCtx && refThreads == o.refThreads && stepMode == o.stepMode && timing == o.timing;
+		}
+	};
+
 	struct Context
 	{
 		Engine* e = nullptr;
@@ -165,11 +177,11 @@ namespace wsp
 		CUtensorMap mapQ, mapK, mapVt;
 		int bnD = 128, bn3D = 128, bn4D = 128, bnCross = 128;
 
-		// persistent decoder-step kernel (decode_mega.cu): per-layer pointer table on the device, grid-barrier counter
-		kern::MegaLayer* megaLayers = nullptr;
+		// per-layer pointer table of both decoder-step kernels, on the device
+		kern::DecStepLayer* stepLayers = nullptr;
+		// persistent decoder-step kernel (decode_mega.cu): grid-barrier counter
 		unsigned* megaBarrier = nullptr;
-		// dataflow decoder-step kernel (decode_flow.cu): per-layer pointer table, per-CTA bias slabs, exchange buffers, launch epoch
-		kern::FlowLayer* flowLayers = nullptr;
+		// dataflow decoder-step kernel (decode_flow.cu): per-CTA bias slabs, exchange buffers, launch epoch
 		float* flowBias = nullptr;
 		uint8_t* flowExch = nullptr;
 		unsigned* flowCtrl = nullptr;
@@ -182,8 +194,7 @@ namespace wsp
 
 		// decode CUDA graph (N = 1 steady state)
 		cudaGraphExec_t stepGraph = nullptr;
-		int stepGraphBatch = 0;
-		int stepGraphCtx = 0;           // encCtx the graph was captured for (the step kernels take it by value)
+		StepGraphKey stepGraphKey;      // what stepGraph was captured for
 		int stepGraphLaunches = 0;
 		bool useGraph = true;
 
