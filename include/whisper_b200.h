@@ -213,6 +213,7 @@ wsp_status wsp_profile_decode( wsp_context* c, int32_t batch, int32_t n_steps, f
  *   "enc.attn"             [n][d]       f16 attention output (head h in columns [64h, 64h + 64))
  *   "enc.h"                [n][4d]      f16 MLP hidden gelu(LN2(x) W1^T + b1) of the last encoded layer
  *   "cross_k", "cross_v"   [L][H][n][64] f16 cross-attention memories (K scaled by 64^-0.25)
+ *   "self_k", "self_v"     [L][H][n_text_ctx][64] f16 decoder self-KV cache (K scaled by 64^-0.25); row j = text position j
  *   "dec.x"                [8][d]       f32 decoder residual stream (shared by all slots) */
 wsp_status wsp_get_tensor( wsp_context* c, const char* name, int32_t slot, float* dst, size_t cap_floats, size_t* n_floats );
 /* debug: run only the first n encoder layers (negative = all) */

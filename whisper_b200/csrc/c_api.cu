@@ -322,6 +322,25 @@ wsp_status wsp_get_tensor( wsp_context* cc, const char* name, int32_t slot, floa
 		}
 		return WSP_OK;
 	}
+	else if( nm == "self_k" || nm == "self_v" )
+	{
+		// gathered per layer: [L][H][n_text_ctx][64] of this slot (the decoder's self-KV cache, head-major rows)
+		const size_t slab = (size_t)hp.n_text_ctx * hp.n_text_state;
+		n = (size_t)L * slab;
+		*n_floats = n;
+		if( !dst ) return WSP_OK;
+		if( cap < n ) return fail( WSP_E_BOUNDS, "dst too small" );
+		DevTmp<float> tmp;
+		WSP_CUDA( tmp.alloc( slab ) );
+		const __half* base = nm == "self_k" ? c.selfK : c.selfV;
+		for( int l = 0; l < L; l++ )
+		{
+			const __half* src = base + ( (size_t)l * c.maxB + slot ) * slab;
+			half_to_float_kernel<<<(unsigned)( ( slab + 255 ) / 256 ), 256>>>( src, tmp.p, slab );
+			WSP_CUDA( cudaMemcpy( dst + (size_t)l * slab, tmp.p, slab * 4, cudaMemcpyDeviceToHost ) );
+		}
+		return WSP_OK;
+	}
 	else if( nm == "dec.x" ) { f32 = c.xd; n = (size_t)d * 8; }
 	else return fail( WSP_E_INVALIDARG, "unknown tensor name " + nm );
 	*n_floats = n;
