@@ -18,6 +18,7 @@
  *                             (Whisper/Whisper/WhisperContext.cpp:578 decode, Whisper/Whisper/ContextImpl.cpp:71-157 sampleBest)
  *   wsp_get_logits/probs      Whisper/source/whisper.h:166 whisper_get_probs
  *   wsp_run_chunks            the fixed-length greedy chunk loop of BASELINE.md §2 (mel + encode + n_decode x (decode + sample))
+ *   wsp_run_chunks_until_eot  the same loop, each chunk cut at its first EOT and the batch stopped soon after its last one
  *   wsp_get_tensor            the reference's named trace points, Whisper/Utils/Trace/tracing.h (names as in whisper.cpp:1121-1869)
  *
  * Error handling mirrors the reference's HRESULT convention (SURVEY.md §8b): every function returns a wsp_status that the COM
@@ -168,6 +169,17 @@ wsp_status wsp_run_chunks( wsp_context* c, const float* const* pcm, const int32_
 wsp_status wsp_upload_pcm( wsp_context* c, int32_t slot, const float* pcm, int32_t n_samples );
 /* ... and run the same path from it: mel + encode + decode with no host->device input copy inside (bench.py's `value` leg) */
 wsp_status wsp_run_chunks_resident( wsp_context* c, int32_t batch, const int32_t* prompt, int32_t n_prompt, int32_t n_decode, int32_t* tokens_out, float* stage_ms );
+/* The batch path of wsp_run_chunks, ending each chunk at its first EOT: chunk b's output is its greedy tokens up to and including
+ * the first EOT, or max_decode tokens if it samples none; n_out[b] = that count; tokens_out[b*max_decode + i] for i < n_out[b]
+ * (tokens_out may be NULL; entries past n_out[b] are not written).  EOT and max_decode are the only stop rules: whisper_full's others
+ * (a timestamp past the window's end, max_tokens) do not apply.  A chunk that has ended stays in the batch and keeps being decoded
+ * until the batch stops; its later tokens are not part of its output.  The steps go out in blocks of 8 and the host reads the
+ * number of ended chunks one block behind, so the batch stops at most 16 steps after its last chunk's EOT.
+ * pcm == NULL runs from the slots' resident PCM (wsp_upload_pcm), as wsp_run_chunks_resident does; otherwise n_samples is required.
+ * Bounds, errors and stage_ms are those of wsp_run_chunks; stage_ms[2] covers the steps actually run, and afterwards wsp_get_logits
+ * and wsp_get_tensor("self_k" / "self_v") hold the state of the last of them. */
+wsp_status wsp_run_chunks_until_eot( wsp_context* c, const float* const* pcm, const int32_t* n_samples, int32_t batch,
+	const int32_t* prompt, int32_t n_prompt, int32_t max_decode, int32_t* tokens_out, int32_t* n_out, float* stage_ms );
 
 /* ---- several devices in one process (csrc/replicas.cpp) ----
  * Chunks are independent (SURVEY.md §8e): one engine + context per listed device (a device may be listed twice: two contexts on one

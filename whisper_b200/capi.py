@@ -37,7 +37,7 @@ EXPORTS = [
     "wsp_engine_create", "wsp_engine_create_from_image", "wsp_engine_destroy", "wsp_engine_weight_bytes",
     "wsp_context_create", "wsp_context_destroy", "wsp_synchronize",
     "wsp_context_device_bytes", "wsp_pcm_to_mel", "wsp_pcm_to_mel_window", "wsp_set_mel", "wsp_mel_len", "wsp_get_mel", "wsp_encode", "wsp_set_audio_ctx", "wsp_set_speed_up", "wsp_decode", "wsp_get_logits", "wsp_get_probs",
-    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_upload_pcm", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
+    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_run_chunks_until_eot", "wsp_upload_pcm", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
     "wsp_host_alloc", "wsp_host_free", "wsp_timings",
     "wsp_replicas_create", "wsp_replicas_count", "wsp_replicas_run_chunks", "wsp_replicas_debug_fail_next", "wsp_replicas_destroy",
     "wsp_test_gemm", "wsp_test_attention", "wsp_test_skinny", "wsp_test_layernorm", "wsp_test_sample",
@@ -102,6 +102,7 @@ def lib():
     sig("wsp_get_probs", i32, [vp, fp, sz])
     sig("wsp_run_chunks", i32, [vp, C.POINTER(fp), ip, i32, ip, i32, i32, ip, fp])
     sig("wsp_run_chunks_resident", i32, [vp, i32, ip, i32, i32, ip, fp])
+    sig("wsp_run_chunks_until_eot", i32, [vp, C.POINTER(fp), ip, i32, ip, i32, i32, ip, ip, fp])
     sig("wsp_upload_pcm", i32, [vp, i32, fp, i32])
     sig("wsp_timer_start", i32, [vp])
     sig("wsp_timer_stop", i32, [vp, fp])
@@ -332,6 +333,22 @@ class Context:
         st = np.zeros(3, np.float32)
         check(self.L.wsp_run_chunks_resident(self.h, batch, _i(pr), pr.size, n_decode, _i(toks), _f(st)))
         return toks, st
+
+    def run_chunks_until_eot(self, pcms, prompt, max_decode: int, batch: int | None = None):
+        """Each chunk's greedy tokens up to and including its first EOT (at most max_decode).  pcms: list of float32 arrays, or
+        None to run `batch` chunks from the slots' resident PCM (upload_pcm).  Returns (list of token arrays, stage_ms[3])."""
+        ptrs, ns = None, None
+        if pcms is not None:
+            batch = len(pcms)
+            arrs = [np.ascontiguousarray(p, np.float32) for p in pcms]
+            ptrs = (C.POINTER(C.c_float) * batch)(*[_f(a) for a in arrs])
+            ns = np.array([a.size for a in arrs], np.int32)
+        pr = np.ascontiguousarray(prompt, np.int32)
+        toks = np.zeros((batch, max_decode), np.int32)
+        n_out = np.zeros(batch, np.int32)
+        st = np.zeros(3, np.float32)
+        check(self.L.wsp_run_chunks_until_eot(self.h, ptrs, None if ns is None else _i(ns), batch, _i(pr), pr.size, max_decode, _i(toks), _i(n_out), _f(st)))
+        return [toks[b, :n_out[b]].copy() for b in range(batch)], st
 
     def upload_pcm(self, slot: int, pcm: np.ndarray):
         pcm = np.ascontiguousarray(pcm, np.float32)

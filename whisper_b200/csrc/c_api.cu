@@ -239,12 +239,22 @@ wsp_status wsp_run_chunks( wsp_context* c, const float* const* pcm, const int32_
 	int32_t n_decode, int32_t* tokens_out, float* stage_ms )
 {
 	if( !c ) return fail( WSP_E_POINTER, "context" );
-	return guarded( [ & ]() -> wsp_status { return ctxRunChunks( *c->c, pcm, n_samples, batch, prompt, n_prompt, n_decode, tokens_out, stage_ms, false ); } );
+	return guarded( [ & ]() -> wsp_status { return ctxRunChunks( *c->c, pcm, n_samples, batch, prompt, n_prompt, n_decode, tokens_out, nullptr, stage_ms, false ); } );
 }
 wsp_status wsp_run_chunks_resident( wsp_context* c, int32_t batch, const int32_t* prompt, int32_t n_prompt, int32_t n_decode, int32_t* tokens_out, float* stage_ms )
 {
 	if( !c ) return fail( WSP_E_POINTER, "context" );
-	return guarded( [ & ]() -> wsp_status { return ctxRunChunks( *c->c, nullptr, nullptr, batch, prompt, n_prompt, n_decode, tokens_out, stage_ms, true ); } );
+	return guarded( [ & ]() -> wsp_status { return ctxRunChunks( *c->c, nullptr, nullptr, batch, prompt, n_prompt, n_decode, tokens_out, nullptr, stage_ms, true ); } );
+}
+wsp_status wsp_run_chunks_until_eot( wsp_context* c, const float* const* pcm, const int32_t* n_samples, int32_t batch, const int32_t* prompt,
+	int32_t n_prompt, int32_t max_decode, int32_t* tokens_out, int32_t* n_out, float* stage_ms )
+{
+	if( !c ) return fail( WSP_E_POINTER, "context" );
+	if( !n_out ) return fail( WSP_E_POINTER, "n_out" );
+	if( pcm && !n_samples ) return fail( WSP_E_POINTER, "n_samples" );
+	return guarded( [ & ]() -> wsp_status {
+		return ctxRunChunks( *c->c, pcm, n_samples, batch, prompt, n_prompt, max_decode, tokens_out, n_out, stage_ms, pcm == nullptr );
+	} );
 }
 
 wsp_status wsp_upload_pcm( wsp_context* c, int32_t slot, const float* pcm, int32_t n_samples )

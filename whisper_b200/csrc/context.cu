@@ -37,9 +37,11 @@ namespace wsp
 		for( auto& v : prof.pool ) cudaEventDestroy( v );
 		for( auto& v : timerEv ) if( v ) cudaEventDestroy( v );
 		void* bufs[] = { stepLayers, flowBias, flowExch, flowCtrl, megaBarrier, stepMarks, melMax, pcmDev, melF16, conv1, x, xn, q, k, vt, attn, h, crossK, crossV, selfK, selfV, xd, qd, attnD, hD, logits, probs, tieScratch,
-			tokensDev, dNPast, sampled, history };
+			tokensDev, dNPast, sampled, history, endStep };
 		for( void* b : bufs ) if( b ) cudaFree( b );
+		if( nEndedHost ) cudaFreeHost( nEndedHost );
 		for( auto& v : ev ) if( v ) cudaEventDestroy( v );
+		for( auto& v : blockEv ) if( v ) cudaEventDestroy( v );
 		if( stream ) cudaStreamDestroy( stream );
 	}
 
@@ -61,6 +63,7 @@ namespace wsp
 		WSP_CUDA( cudaStreamCreateWithFlags( &c.stream, cudaStreamNonBlocking ) );
 		for( auto& v : c.ev ) WSP_CUDA( cudaEventCreate( &v ) );
 		for( auto& v : c.timerEv ) WSP_CUDA( cudaEventCreate( &v ) );
+		for( auto& v : c.blockEv ) WSP_CUDA( cudaEventCreateWithFlags( &v, cudaEventDisableTiming ) );
 		c.slots.resize( maxBatch );
 		const size_t B = (size_t)maxBatch;
 		WSP_CHECK( devAlloc( c.melMax, B ) );
@@ -89,9 +92,14 @@ namespace wsp
 		WSP_CHECK( devAlloc( c.dNPast, 8, true ) );
 		c.dFlags = c.dNPast + 2;
 		c.dStep = c.dNPast + 4;
+		c.nEnded = c.dNPast + 6;
 		WSP_CHECK( devAlloc( c.sampled, B ) );
 		c.histCap = hp.n_text_ctx;
 		WSP_CHECK( devAlloc( c.history, B * c.histCap, true ) );
+		WSP_CHECK( devAlloc( c.endStep, B, true ) );
+		WSP_CUDA( cudaHostAlloc( (void**)&c.nEndedHost, sizeof( int ), cudaHostAllocMapped ) );
+		*c.nEndedHost = 0;
+		WSP_CUDA( cudaHostGetDevicePointer( (void**)&c.nEndedMapped, c.nEndedHost, 0 ) );
 
 		// ---- tensor maps ----
 		c.bnD = pickBN( d ); c.bn3D = pickBN( 3 * d ); c.bn4D = pickBN( 4 * d ); c.bnCross = pickBN( L * 2 * d );
@@ -476,6 +484,7 @@ namespace wsp
 		sa.tokenBeg = e.tokBeg; sa.tokenSot = e.tokSot; sa.tokenSolm = e.tokSolm; sa.tokenNot = e.tokNot;
 		sa.dForceTs = c.dFlags; sa.out = c.sampled; sa.nextTokens = c.tokensDev; sa.dNPast = c.dNPast; sa.N = N;
 		sa.history = c.history; sa.histCap = c.histCap; sa.dStep = c.dStep;
+		if( c.eotArmed ) { sa.tokenEot = e.tokEot; sa.endStep = c.endStep; sa.nEnded = c.nEnded; sa.nEndedHost = c.nEndedMapped; }
 		WSP_KERNEL( KK_OTHER, kern::sampleGreedy( sa, c.stream ) );
 		return WSP_OK;
 	}
@@ -578,7 +587,7 @@ namespace wsp
 		int n = 0;
 		if( N == 1 && !allLogits && sample && c.useGraph && !c.prof.on )
 		{
-			const StepGraphKey key{ batch, c.encCtx, c.refThreads, c.stepMode, c.stepTiming };
+			const StepGraphKey key{ batch, c.encCtx, c.refThreads, c.stepMode, c.stepTiming, c.eotArmed };
 			if( !c.stepGraph || !( c.stepGraphKey == key ) )
 			{
 				if( c.stepGraph ) { cudaGraphExecDestroy( c.stepGraph ); c.stepGraph = nullptr; }
@@ -696,14 +705,20 @@ namespace wsp
 	// ===============================================================================================================
 	// the measured path: mel + encode + n_decode greedy steps, tokens fed back on the device
 	// ===============================================================================================================
+	// steps per block of wsp_run_chunks_until_eot: the host checks block k - 1's end-of-text count while block k runs
+	constexpr int kEotLag = 8;
+
 	int ctxRunChunks( Context& c, const float* const* pcm, const int32_t* nSamples, int batch, const int32_t* prompt, int nPrompt, int nDecode,
-		int32_t* tokensOut, float* stageMs, bool resident )
+		int32_t* tokensOut, int32_t* nOut, float* stageMs, bool resident )
 	{
 		const HParams& hp = c.e->hp;
 		if( batch < 1 || batch > c.maxB ) return fail( WSP_E_BOUNDS, "batch exceeds the context's max_batch" );
 		if( !prompt || nPrompt < 1 || nPrompt > kMaxDecodeTokens ) return fail( WSP_E_INVALIDARG, "prompt" );
 		if( nDecode < 1 || nPrompt + nDecode > hp.n_text_ctx || nDecode > c.histCap ) return fail( WSP_E_BOUNDS, "n_prompt + n_decode exceeds n_text_ctx" );
 		if( !resident && ( !pcm || !nSamples ) ) return fail( WSP_E_POINTER, "pcm" );
+		if( !resident )
+			for( int b = 0; b < batch; b++ ) if( nSamples[ b ] < 0 ) return fail( WSP_E_INVALIDARG, "n_samples" );
+		const bool untilEot = nOut != nullptr;
 		WSP_CUDA( cudaSetDevice( c.e->device ) );
 		cudaStream_t s = c.stream;
 		WSP_CUDA( cudaEventRecord( c.ev[ 0 ], s ) );
@@ -717,7 +732,7 @@ namespace wsp
 		else
 		{
 			size_t total = 0;
-			for( int b = 0; b < batch; b++ ) { if( nSamples[ b ] < 0 ) return fail( WSP_E_INVALIDARG, "n_samples" ); total += (size_t)nSamples[ b ]; }
+			for( int b = 0; b < batch; b++ ) total += (size_t)nSamples[ b ];
 			WSP_CHECK( ensurePcm( c, total ? total : 1 ) );
 			std::vector<size_t> offs( (size_t)batch );
 			size_t off = 0;
@@ -741,22 +756,54 @@ namespace wsp
 		WSP_CUDA( kern::setInts( c.dFlags, 1, 1, s ) );
 		WSP_CUDA( kern::setInts( c.dStep, 0, 0, s ) );
 		launched( 3 );
-		WSP_CHECK( decodeSubmit( c, nPrompt, batch, false, true ) );
-		for( int i = 1; i < nDecode; i++ )
-			WSP_CHECK( decodeSubmit( c, 1, batch, false, true ) );
-		c.nPastHost = nPrompt + nDecode - 1;
+		int steps = nDecode;
+		if( !untilEot )
+		{
+			WSP_CHECK( decodeSubmit( c, nPrompt, batch, false, true ) );
+			for( int i = 1; i < nDecode; i++ )
+				WSP_CHECK( decodeSubmit( c, 1, batch, false, true ) );
+		}
+		else
+		{
+			// the sampler logs every chunk's first EOT; the steps go out in blocks of kEotLag, and block k is enqueued before the host
+			// waits for block k - 1 and reads how many chunks have ended, so the stream never runs dry between blocks
+			struct Arm { Context& c; Arm( Context& x ) : c( x ) { c.eotArmed = true; } ~Arm() { c.eotArmed = false; } } arm( c );
+			*(volatile int*)c.nEndedHost = 0;
+			WSP_CUDA( cudaMemsetAsync( c.endStep, 0, (size_t)batch * 4, s ) );
+			WSP_CUDA( cudaMemsetAsync( c.nEnded, 0, 4, s ) );
+			WSP_CHECK( decodeSubmit( c, nPrompt, batch, false, true ) );
+			steps = 1;
+			int waitOn = 0;
+			WSP_CUDA( cudaEventRecord( c.blockEv[ waitOn ], s ) );
+			while( steps < nDecode )
+			{
+				const int n = nDecode - steps < kEotLag ? nDecode - steps : kEotLag;
+				for( int i = 0; i < n; i++ ) WSP_CHECK( decodeSubmit( c, 1, batch, false, true ) );
+				steps += n;
+				WSP_CUDA( cudaEventRecord( c.blockEv[ waitOn ^ 1 ], s ) );
+				WSP_CUDA( cudaEventSynchronize( c.blockEv[ waitOn ] ) );
+				waitOn ^= 1;
+				if( *(volatile int*)c.nEndedHost >= batch ) break;
+			}
+		}
+		c.nPastHost = nPrompt + steps - 1;
 		WSP_CUDA( cudaEventRecord( c.ev[ 3 ], s ) );
 		c.lastLogitRows = batch;
-		// one D2H of the token log at the end: [batch][n_decode] int32
-		std::vector<int32_t> hist( (size_t)batch * c.histCap );
+		// one D2H of the token log (and of the end-of-text steps) at the end: [batch][n_decode] int32
+		std::vector<int32_t> hist( (size_t)batch * c.histCap ), ends( (size_t)batch );
 		WSP_CUDA( cudaMemcpyAsync( hist.data(), c.history, hist.size() * 4, cudaMemcpyDeviceToHost, s ) );
+		if( untilEot ) WSP_CUDA( cudaMemcpyAsync( ends.data(), c.endStep, ends.size() * 4, cudaMemcpyDeviceToHost, s ) );
 		WSP_CUDA( cudaStreamSynchronize( s ) );
-		if( tokensOut )
-			for( int b = 0; b < batch; b++ )
-				for( int i = 0; i < nDecode; i++ ) tokensOut[ (size_t)b * nDecode + i ] = hist[ (size_t)b * c.histCap + i ];
+		for( int b = 0; b < batch; b++ )
+		{
+			const int n = untilEot && ends[ (size_t)b ] > 0 ? ends[ (size_t)b ] : nDecode;
+			if( nOut ) nOut[ b ] = n;
+			if( tokensOut )
+				for( int i = 0; i < n; i++ ) tokensOut[ (size_t)b * nDecode + i ] = hist[ (size_t)b * c.histCap + i ];
+		}
 		const float m0 = addStage( c, 0, c.ev[ 0 ], c.ev[ 1 ], 1 );
 		const float m1 = addStage( c, 1, c.ev[ 1 ], c.ev[ 2 ], 1 );
-		const float m2 = addStage( c, 2, c.ev[ 2 ], c.ev[ 3 ], nDecode );
+		const float m2 = addStage( c, 2, c.ev[ 2 ], c.ev[ 3 ], steps );
 		if( stageMs ) { stageMs[ 0 ] = m0; stageMs[ 1 ] = m1; stageMs[ 2 ] = m2; }
 		return WSP_OK;
 	}

@@ -113,9 +113,10 @@ namespace wsp
 	{
 		int batch = 0, encCtx = 0, refThreads = 0, stepMode = 0;
 		bool timing = false;
+		bool eot = false;
 		bool operator==( const StepGraphKey& o ) const
 		{
-			return batch == o.batch && encCtx == o.encCtx && refThreads == o.refThreads && stepMode == o.stepMode && timing == o.timing;
+			return batch == o.batch && encCtx == o.encCtx && refThreads == o.refThreads && stepMode == o.stepMode && timing == o.timing && eot == o.eot;
 		}
 	};
 
@@ -165,6 +166,13 @@ namespace wsp
 		kern::TokenData* sampled = nullptr;   // [maxB]
 		int* history = nullptr;         // [maxB][histCap]
 		int histCap = 0;
+		// end-of-text log of wsp_run_chunks_until_eot: the sampler fills it only while eotArmed is set
+		bool eotArmed = false;
+		int* endStep = nullptr;         // [maxB] 1 + the step of each chunk's first EOT, 0 = none yet
+		int* nEnded = nullptr;          // device counter of chunks with an EOT (in the dNPast block)
+		int* nEndedHost = nullptr;      // mapped pinned copy of nEnded, written by the last kernel of every step
+		int* nEndedMapped = nullptr;    // its device address
+		cudaEvent_t blockEv[ 2 ] = { nullptr, nullptr };   // ends of the last two enqueued step blocks
 		int lastLogitRows = 0;
 		int nPastHost = 0;              // host mirror of the device-resident n_past (it advances on the device between graph replays)
 		int debugEncLayers = -1;
@@ -219,5 +227,7 @@ namespace wsp
 	int ctxDecode( Context& c, const int32_t* tokensHost, int nTokens, int nPast, int batch, uint32_t flags, wsp_token_data* sampledHost );
 	int ctxUploadPcm( Context& c, int slot, const float* pcmHost, int nSamples );
 	int ctxProfileDecode( Context& c, int batch, int nSteps, float* msByKind, int* launchesByKind );
-	int ctxRunChunks( Context& c, const float* const* pcm, const int32_t* nSamples, int batch, const int32_t* prompt, int nPrompt, int nDecode, int32_t* tokensOut, float* stageMs, bool resident );
+	// nOut == nullptr: nDecode steps for every chunk (wsp_run_chunks*); else each chunk ends at its first EOT (wsp_run_chunks_until_eot)
+	int ctxRunChunks( Context& c, const float* const* pcm, const int32_t* nSamples, int batch, const int32_t* prompt, int nPrompt, int nDecode,
+		int32_t* tokensOut, int32_t* nOut, float* stageMs, bool resident );
 }

@@ -125,6 +125,12 @@ namespace kern
 		int histCap = 0;
 		int* dStep = nullptr;
 		int* tieScratch = nullptr;      // required: [B][nVocab + 1024] ints, survivor lists of the exact tie emulation
+		// end-of-text log (null = unarmed): the first time row b samples tokenEot, endStep[b] (zeroed by the caller) = *dStep + 1
+		// and *nEnded is incremented; the advance kernel then copies *nEnded to *nEndedHost (mapped pinned host memory)
+		int tokenEot = 0;
+		int* endStep = nullptr;
+		int* nEnded = nullptr;
+		volatile int* nEndedHost = nullptr;
 	};
 	// one cluster of 4 CTAs per row (any nVocab >= 8 whose quarter fits shared memory), then the 1-thread advance of n_past / flags / step
 	cudaError_t sampleGreedy( const SampleArgs& a, cudaStream_t s );

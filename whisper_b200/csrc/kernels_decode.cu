@@ -672,6 +672,11 @@ namespace kern
 			a.out[ b ] = td;
 			if( a.nextTokens ) a.nextTokens[ b ] = td.id;
 			if( a.history && a.dStep && *a.dStep < a.histCap ) a.history[ (size_t)b * a.histCap + *a.dStep ] = td.id;
+			if( a.endStep && td.id == a.tokenEot && a.endStep[ b ] == 0 )
+			{
+				a.endStep[ b ] = *a.dStep + 1;
+				atomicAdd( a.nEnded, 1 );
+			}
 		}
 		}
 		cluster.sync();   // nobody leaves while a peer may still read its partials
@@ -705,13 +710,15 @@ namespace kern
 		return cudaGetLastError();
 	}
 
-	__global__ void advance_kernel( int* dNPast, int N, int* dForceTs, int* dStep )
+	__global__ void advance_kernel( int* dNPast, int N, int* dForceTs, int* dStep, const int* nEnded, volatile int* nEndedHost )
 	{
 		ptx::pdl_launch_dependents();
 		ptx::pdl_wait();
 		if( dNPast ) *dNPast += N;
 		if( dForceTs ) { dForceTs[ 0 ] = 0; dForceTs[ 1 ] = 0; }
 		if( dStep ) *dStep += 1;
+		// one writer after the whole sampler grid: the host never sees the counter go backwards
+		if( nEndedHost ) *nEndedHost = *nEnded;
 	}
 
 	cudaError_t sampleGreedy( const SampleArgs& a, cudaStream_t s )
@@ -736,6 +743,8 @@ namespace kern
 		e = cudaLaunchKernelEx( &cfg, sample_cluster_kernel<CL>, a );
 		if( e != cudaSuccess ) return e;
 		// step-global state is advanced by a separate 1-thread kernel so that no CTA of the sampler races with it
-		return launchPdl( advance_kernel, dim3( 1 ), dim3( 1 ), 0, s, a.dNPast, a.N, const_cast<int*>( a.dForceTs ), a.dStep );
+		if( a.endStep && ( !a.nEnded || !a.nEndedHost ) ) return cudaErrorInvalidValue;
+		return launchPdl( advance_kernel, dim3( 1 ), dim3( 1 ), 0, s, a.dNPast, a.N, const_cast<int*>( a.dForceTs ), a.dStep,
+			(const int*)a.nEnded, a.endStep ? a.nEndedHost : (volatile int*)nullptr );
 	}
 }
