@@ -19,6 +19,7 @@
  *   wsp_get_logits/probs      Whisper/source/whisper.h:166 whisper_get_probs
  *   wsp_run_chunks            the fixed-length greedy chunk loop of BASELINE.md §2 (mel + encode + n_decode x (decode + sample))
  *   wsp_run_chunks_until_eot  the same loop, each chunk cut at its first EOT and the batch stopped soon after its last one
+ *   wsp_get_chunk_languages   whisper_lang_auto_detect (Whisper/source/whisper.cpp:2428-2495) per chunk of a run_chunks* call
  *   wsp_get_tensor            the reference's named trace points, Whisper/Utils/Trace/tracing.h (names as in whisper.cpp:1121-1869)
  *
  * Error handling mirrors the reference's HRESULT convention (SURVEY.md §8b): every function returns a wsp_status that the COM
@@ -160,6 +161,16 @@ wsp_status wsp_get_probs( wsp_context* c, float* dst, size_t cap_floats );
  * then — like the reference — a softmax over the language tokens' PROBABILITIES; lang_probs[n_langs] (nullable), *lang_id = the arg-max */
 wsp_status wsp_detect_language( wsp_context* c, int32_t offset_frames, int32_t n_langs, float* lang_probs, int32_t* lang_id );
 
+/* Prompt token of wsp_run_chunks, wsp_run_chunks_resident and wsp_run_chunks_until_eot (and of wsp_replicas_run_chunks, which passes
+ * its prompt through): "detect this chunk's language".  A prompt may hold it at most once, e.g. [sot, WSP_TOKEN_LANGUAGE_AUTO, transcribe].
+ * The call then detects each chunk's language from that chunk's own encode, as whisper_lang_auto_detect does at offset 0 (one decoder
+ * pass over [sot] for the whole batch, the reference's softmax over the language tokens' probabilities, arg-max), and decodes chunk b
+ * with the sentinel replaced by its language token sot + 1 + lang_b.  The languages considered are the n_langs = translate - sot - 1
+ * tokens after sot (99 on the multilingual vocabulary); on a model that is not multilingual the sentinel is WSP_E_INVALIDARG.  Detection
+ * sees the context's current audio_ctx and speed-up, like the batch's own encode; stage_ms[2] includes it.  Every other prompt id
+ * must satisfy 0 <= id < n_vocab, else the call is WSP_E_INVALIDARG and launches nothing. */
+enum { WSP_TOKEN_LANGUAGE_AUTO = -1 };
+
 /* The measured path: for `batch` chunks of host PCM — mel, encode, then n_decode greedy steps (first step samples with
  * is_initial timestamp rules, as whisper_full does, whisper.cpp:2943) entirely on the device with sampled tokens fed back
  * without host round trips.  tokens_out[b*n_decode + i].  stage_ms (nullable): { h2d+mel, encode, decode } from CUDA events. */
@@ -180,6 +191,12 @@ wsp_status wsp_run_chunks_resident( wsp_context* c, int32_t batch, const int32_t
  * and wsp_get_tensor("self_k" / "self_v") hold the state of the last of them. */
 wsp_status wsp_run_chunks_until_eot( wsp_context* c, const float* const* pcm, const int32_t* n_samples, int32_t batch,
 	const int32_t* prompt, int32_t n_prompt, int32_t max_decode, int32_t* tokens_out, int32_t* n_out, float* stage_ms );
+/* The languages the last wsp_run_chunks* call on this context detected, when its prompt held WSP_TOKEN_LANGUAGE_AUTO: lang_ids[batch]
+ * as wsp_detect_language reports them (0 = en; chunk b's language token is sot + 1 + lang_ids[b]) and, if lang_probs is not NULL,
+ * lang_probs[b*n_langs + l] for b < batch, which needs cap_floats >= batch * n_langs.  They come back with that call's tokens.
+ * WSP_S_FALSE, writing nothing, when that call had no sentinel (or there was none); WSP_E_BOUNDS for a batch above that call's or a
+ * short cap_floats. */
+wsp_status wsp_get_chunk_languages( wsp_context* c, int32_t batch, int32_t* lang_ids, float* lang_probs, size_t cap_floats );
 
 /* ---- several devices in one process (csrc/replicas.cpp) ----
  * Chunks are independent (SURVEY.md §8e): one engine + context per listed device (a device may be listed twice: two contexts on one

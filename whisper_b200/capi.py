@@ -14,6 +14,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libwhisper_b200.so")
 
 WSP_OK = 0
+WSP_S_FALSE = 1
+TOKEN_LANGUAGE_AUTO = -1   # WSP_TOKEN_LANGUAGE_AUTO: the prompt slot of each chunk's detected language (run_chunks*)
 DECODE_FORCE_TIMESTAMP = 1
 DECODE_INITIAL = 2
 DECODE_ALL_LOGITS = 4
@@ -37,7 +39,7 @@ EXPORTS = [
     "wsp_engine_create", "wsp_engine_create_from_image", "wsp_engine_destroy", "wsp_engine_weight_bytes",
     "wsp_context_create", "wsp_context_destroy", "wsp_synchronize",
     "wsp_context_device_bytes", "wsp_pcm_to_mel", "wsp_pcm_to_mel_window", "wsp_set_mel", "wsp_mel_len", "wsp_get_mel", "wsp_encode", "wsp_set_audio_ctx", "wsp_set_speed_up", "wsp_decode", "wsp_get_logits", "wsp_get_probs",
-    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_run_chunks_until_eot", "wsp_upload_pcm", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
+    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_run_chunks_until_eot", "wsp_get_chunk_languages", "wsp_upload_pcm", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
     "wsp_host_alloc", "wsp_host_free", "wsp_timings",
     "wsp_replicas_create", "wsp_replicas_count", "wsp_replicas_run_chunks", "wsp_replicas_debug_fail_next", "wsp_replicas_destroy",
     "wsp_test_gemm", "wsp_test_attention", "wsp_test_skinny", "wsp_test_layernorm", "wsp_test_sample",
@@ -103,6 +105,7 @@ def lib():
     sig("wsp_run_chunks", i32, [vp, C.POINTER(fp), ip, i32, ip, i32, i32, ip, fp])
     sig("wsp_run_chunks_resident", i32, [vp, i32, ip, i32, i32, ip, fp])
     sig("wsp_run_chunks_until_eot", i32, [vp, C.POINTER(fp), ip, i32, ip, i32, i32, ip, ip, fp])
+    sig("wsp_get_chunk_languages", i32, [vp, i32, ip, fp, sz])
     sig("wsp_upload_pcm", i32, [vp, i32, fp, i32])
     sig("wsp_timer_start", i32, [vp])
     sig("wsp_timer_stop", i32, [vp, fp])
@@ -203,11 +206,12 @@ class Model:
             self.L.wsp_model_close(self.h)
             self.h = None
 
-    def prompt_init(self, language_id: int = 0, translate: bool = False):
-        """[sot, (lang, task)] as whisper_full builds it (whisper.cpp:2839-2848)."""
+    def prompt_init(self, language_id: int | str = 0, translate: bool = False):
+        """[sot, (lang, task)] as whisper_full builds it (whisper.cpp:2839-2848).  language_id="auto" puts TOKEN_LANGUAGE_AUTO in the
+        language slot: run_chunks* then detect each chunk's language (Context.chunk_languages)."""
         p = [self.special["sot"]]
         if self.multilingual:
-            p.append(self.special["sot"] + 1 + language_id)
+            p.append(TOKEN_LANGUAGE_AUTO if language_id == "auto" else self.special["sot"] + 1 + language_id)
             p.append(self.special["translate"] if translate else self.special["transcribe"])
         return p
 
@@ -349,6 +353,16 @@ class Context:
         st = np.zeros(3, np.float32)
         check(self.L.wsp_run_chunks_until_eot(self.h, ptrs, None if ns is None else _i(ns), batch, _i(pr), pr.size, max_decode, _i(toks), _i(n_out), _f(st)))
         return [toks[b, :n_out[b]].copy() for b in range(batch)], st
+
+    def chunk_languages(self, batch: int):
+        """The languages the last run_chunks* call detected for chunks [0, batch) (its prompt held TOKEN_LANGUAGE_AUTO): (ids[batch],
+        probs[batch][n_langs]), ids as detect_language reports them (0 = en).  None if that call had no sentinel."""
+        n_langs = self.model.special["translate"] - self.model.special["sot"] - 1
+        ids = np.zeros(batch, np.int32)
+        probs = np.zeros((batch, n_langs), np.float32)
+        if check(self.L.wsp_get_chunk_languages(self.h, batch, _i(ids), _f(probs), probs.size)) == WSP_S_FALSE:
+            return None
+        return ids, probs
 
     def upload_pcm(self, slot: int, pcm: np.ndarray):
         pcm = np.ascontiguousarray(pcm, np.float32)

@@ -256,6 +256,18 @@ wsp_status wsp_run_chunks_until_eot( wsp_context* c, const float* const* pcm, co
 		return ctxRunChunks( *c->c, pcm, n_samples, batch, prompt, n_prompt, max_decode, tokens_out, n_out, stage_ms, pcm == nullptr );
 	} );
 }
+wsp_status wsp_get_chunk_languages( wsp_context* c, int32_t batch, int32_t* lang_ids, float* lang_probs, size_t cap_floats )
+{
+	if( !c || !lang_ids ) return fail( WSP_E_POINTER, "context/lang_ids" );
+	const Context& cx = *c->c;
+	if( cx.lastLangIds.empty() ) return WSP_S_FALSE;
+	const size_t nLangs = (size_t)cx.e->nLangs;
+	if( batch < 0 || (size_t)batch > cx.lastLangIds.size() ) return fail( WSP_E_BOUNDS, "batch exceeds the last call's batch" );
+	if( lang_probs && cap_floats < (size_t)batch * nLangs ) return fail( WSP_E_BOUNDS, "lang_probs too small" );
+	std::copy( cx.lastLangIds.begin(), cx.lastLangIds.begin() + batch, lang_ids );
+	if( lang_probs ) std::copy( cx.lastLangProbs.begin(), cx.lastLangProbs.begin() + (size_t)batch * nLangs, lang_probs );
+	return WSP_OK;
+}
 
 wsp_status wsp_upload_pcm( wsp_context* c, int32_t slot, const float* pcm, int32_t n_samples )
 {

@@ -37,7 +37,7 @@ namespace wsp
 		for( auto& v : prof.pool ) cudaEventDestroy( v );
 		for( auto& v : timerEv ) if( v ) cudaEventDestroy( v );
 		void* bufs[] = { stepLayers, flowBias, flowExch, flowCtrl, megaBarrier, stepMarks, melMax, pcmDev, melF16, conv1, x, xn, q, k, vt, attn, h, crossK, crossV, selfK, selfV, xd, qd, attnD, hD, logits, probs, tieScratch,
-			tokensDev, dNPast, sampled, history, endStep };
+			tokensDev, dNPast, sampled, history, endStep, langIds, langProbs };
 		for( void* b : bufs ) if( b ) cudaFree( b );
 		if( nEndedHost ) cudaFreeHost( nEndedHost );
 		for( auto& v : ev ) if( v ) cudaEventDestroy( v );
@@ -97,6 +97,11 @@ namespace wsp
 		c.histCap = hp.n_text_ctx;
 		WSP_CHECK( devAlloc( c.history, B * c.histCap, true ) );
 		WSP_CHECK( devAlloc( c.endStep, B, true ) );
+		if( e->nLangs > 0 )
+		{
+			WSP_CHECK( devAlloc( c.langIds, B, true ) );
+			WSP_CHECK( devAlloc( c.langProbs, B * e->nLangs, true ) );
+		}
 		WSP_CUDA( cudaHostAlloc( (void**)&c.nEndedHost, sizeof( int ), cudaHostAllocMapped ) );
 		*c.nEndedHost = 0;
 		WSP_CUDA( cudaHostGetDevicePointer( (void**)&c.nEndedMapped, c.nEndedHost, 0 ) );
@@ -705,6 +710,30 @@ namespace wsp
 	// ===============================================================================================================
 	// the measured path: mel + encode + n_decode greedy steps, tokens fed back on the device
 	// ===============================================================================================================
+	// whisper_lang_auto_detect for every chunk of the batch from its own encode (whisper.cpp:2428-2495): one N = 1 decoder pass over
+	// [sot] at n_past 0 without sampling (the default step kernel; it writes self-KV row 0, which the prompt pass then rewrites), the
+	// vocabulary softmax of the all-logits path, and langPick, which records each chunk's language and writes its prompt to tokensDev.
+	// c.tokensDev[b] = sot and n_past = 0 are the caller's.
+	static int enqueueLanguageDetection( Context& c, int batch, const int32_t* prompt, int nPrompt, int autoPos )
+	{
+		const Engine& e = *c.e;
+		int n = 0;
+		{
+			// the step-timing marks (wsp_debug_step_timing) stay those of the sampled steps: this pass records none
+			struct NoTiming { Context& c; bool was; NoTiming( Context& x ) : c( x ), was( x.stepTiming ) { c.stepTiming = false; } ~NoTiming() { c.stepTiming = was; } } nt( c );
+			WSP_CHECK( decodeEnqueue( c, 1, batch, false, false, &n ) );
+		}
+		WSP_CUDA( kern::softmaxRows( c.logits, c.probs, batch, e.hp.n_vocab, c.stream ) );
+		kern::LangPickArgs la{};
+		la.probs = c.probs; la.nVocab = e.hp.n_vocab; la.tokLang0 = e.tokSot + 1; la.nLangs = e.nLangs;
+		la.langIds = c.langIds; la.langProbs = c.langProbs; la.tokens = c.tokensDev; la.nPrompt = nPrompt; la.autoPos = autoPos;
+		for( int i = 0; i < nPrompt; i++ ) la.tmpl[ i ] = prompt[ i ];
+		WSP_CUDA( kern::langPick( la, batch, c.stream ) );
+		launched( n + 2 );
+		return WSP_OK;
+	}
+	static_assert( kMaxDecodeTokens <= kern::kLangPromptMax, "a prompt template must fit LangPickArgs" );
+
 	// steps per block of wsp_run_chunks_until_eot: the host checks block k - 1's end-of-text count while block k runs
 	constexpr int kEotLag = 8;
 
@@ -714,11 +743,26 @@ namespace wsp
 		const HParams& hp = c.e->hp;
 		if( batch < 1 || batch > c.maxB ) return fail( WSP_E_BOUNDS, "batch exceeds the context's max_batch" );
 		if( !prompt || nPrompt < 1 || nPrompt > kMaxDecodeTokens ) return fail( WSP_E_INVALIDARG, "prompt" );
+		// every id indexes the embedding table, as ctxDecode's tokens do; at most one is the language sentinel
+		int autoPos = -1;
+		for( int i = 0; i < nPrompt; i++ )
+		{
+			if( prompt[ i ] == WSP_TOKEN_LANGUAGE_AUTO )
+			{
+				if( autoPos >= 0 ) return fail( WSP_E_INVALIDARG, "the prompt holds WSP_TOKEN_LANGUAGE_AUTO more than once" );
+				autoPos = i;
+			}
+			else if( prompt[ i ] < 0 || prompt[ i ] >= hp.n_vocab ) return fail( WSP_E_INVALIDARG, "prompt token id out of range" );
+		}
+		const bool detect = autoPos >= 0;
+		if( detect && c.e->nLangs < 1 ) return fail( WSP_E_INVALIDARG, "WSP_TOKEN_LANGUAGE_AUTO needs a multilingual model" );
 		if( nDecode < 1 || nPrompt + nDecode > hp.n_text_ctx || nDecode > c.histCap ) return fail( WSP_E_BOUNDS, "n_prompt + n_decode exceeds n_text_ctx" );
 		if( !resident && ( !pcm || !nSamples ) ) return fail( WSP_E_POINTER, "pcm" );
 		if( !resident )
 			for( int b = 0; b < batch; b++ ) if( nSamples[ b ] < 0 ) return fail( WSP_E_INVALIDARG, "n_samples" );
 		const bool untilEot = nOut != nullptr;
+		c.lastLangIds.clear();
+		c.lastLangProbs.clear();
 		WSP_CUDA( cudaSetDevice( c.e->device ) );
 		cudaStream_t s = c.stream;
 		WSP_CUDA( cudaEventRecord( c.ev[ 0 ], s ) );
@@ -748,14 +792,17 @@ namespace wsp
 		WSP_CUDA( cudaEventRecord( c.ev[ 1 ], s ) );
 		WSP_CHECK( encodeAsync( c, nullptr, batch ) );
 		WSP_CUDA( cudaEventRecord( c.ev[ 2 ], s ) );
-		// prompt step: same prompt for every chunk, first sample uses the initial-timestamp rules (whisper.cpp:2943)
-		std::vector<int32_t> ptoks( (size_t)batch * nPrompt );
-		for( int b = 0; b < batch; b++ ) for( int i = 0; i < nPrompt; i++ ) ptoks[ (size_t)b * nPrompt + i ] = prompt[ i ];
+		// prompt step: same prompt for every chunk, first sample uses the initial-timestamp rules (whisper.cpp:2943); with the
+		// language sentinel the tokens uploaded are the detection pass's [sot] per chunk, and langPick writes the prompts
+		std::vector<int32_t> ptoks( detect ? (size_t)batch : (size_t)batch * nPrompt, c.e->tokSot );
+		if( !detect )
+			for( int b = 0; b < batch; b++ ) for( int i = 0; i < nPrompt; i++ ) ptoks[ (size_t)b * nPrompt + i ] = prompt[ i ];
 		WSP_CUDA( cudaMemcpyAsync( c.tokensDev, ptoks.data(), ptoks.size() * 4, cudaMemcpyHostToDevice, s ) );
 		WSP_CUDA( kern::setInts( c.dNPast, 0, 0, s ) );
 		WSP_CUDA( kern::setInts( c.dFlags, 1, 1, s ) );
 		WSP_CUDA( kern::setInts( c.dStep, 0, 0, s ) );
 		launched( 3 );
+		if( detect ) WSP_CHECK( enqueueLanguageDetection( c, batch, prompt, nPrompt, autoPos ) );
 		int steps = nDecode;
 		if( !untilEot )
 		{
@@ -793,7 +840,16 @@ namespace wsp
 		std::vector<int32_t> hist( (size_t)batch * c.histCap ), ends( (size_t)batch );
 		WSP_CUDA( cudaMemcpyAsync( hist.data(), c.history, hist.size() * 4, cudaMemcpyDeviceToHost, s ) );
 		if( untilEot ) WSP_CUDA( cudaMemcpyAsync( ends.data(), c.endStep, ends.size() * 4, cudaMemcpyDeviceToHost, s ) );
+		std::vector<int32_t> langIds( detect ? (size_t)batch : 0 );
+		std::vector<float> langProbs( detect ? (size_t)batch * c.e->nLangs : 0 );
+		if( detect )
+		{
+			WSP_CUDA( cudaMemcpyAsync( langIds.data(), c.langIds, langIds.size() * 4, cudaMemcpyDeviceToHost, s ) );
+			WSP_CUDA( cudaMemcpyAsync( langProbs.data(), c.langProbs, langProbs.size() * 4, cudaMemcpyDeviceToHost, s ) );
+		}
 		WSP_CUDA( cudaStreamSynchronize( s ) );
+		c.lastLangIds.swap( langIds );
+		c.lastLangProbs.swap( langProbs );
 		for( int b = 0; b < batch; b++ )
 		{
 			const int n = untilEot && ends[ (size_t)b ] > 0 ? ends[ (size_t)b ] : nDecode;

@@ -162,6 +162,8 @@ namespace wsp
 		e->hp = m.hp;
 		e->tokEot = m.vocab.token_eot; e->tokSot = m.vocab.token_sot; e->tokPrev = m.vocab.token_prev;
 		e->tokSolm = m.vocab.token_solm; e->tokNot = m.vocab.token_not; e->tokBeg = m.vocab.token_beg;
+		// the reference's g_lang: language l is token sot + 1 + l, up to the task tokens (whisper.cpp:2466-2468)
+		e->nLangs = m.vocab.multilingual() ? Vocab::token_translate - m.vocab.token_sot - 1 : 0;
 		const HParams& h = m.hp;
 		const int d = h.n_audio_state;
 		const size_t dd = (size_t)d * d;

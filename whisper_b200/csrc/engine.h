@@ -66,6 +66,7 @@ namespace wsp
 		int numSMs = 132;
 		HParams hp{};
 		int tokEot = 0, tokSot = 0, tokPrev = 0, tokSolm = 0, tokNot = 0, tokBeg = 0;
+		int nLangs = 0;                 // language tokens sot + 1 .. sot + nLangs (99 on the multilingual vocabulary, 0 otherwise)
 		uint8_t* arena = nullptr;
 		size_t arenaSize = 0, arenaUsed = 0;
 
@@ -173,6 +174,11 @@ namespace wsp
 		int* nEndedHost = nullptr;      // mapped pinned copy of nEnded, written by the last kernel of every step
 		int* nEndedMapped = nullptr;    // its device address
 		cudaEvent_t blockEv[ 2 ] = { nullptr, nullptr };   // ends of the last two enqueued step blocks
+		// per-chunk language detection of a run_chunks* call whose prompt holds WSP_TOKEN_LANGUAGE_AUTO (lang_pick_kernel)
+		int* langIds = nullptr;         // [maxB]
+		float* langProbs = nullptr;     // [maxB][nLangs]
+		std::vector<int32_t> lastLangIds;   // host copies from the last run_chunks* call (wsp_get_chunk_languages); empty: it had no sentinel
+		std::vector<float> lastLangProbs;   // [batch][nLangs]
 		int lastLogitRows = 0;
 		int nPastHost = 0;              // host mirror of the device-resident n_past (it advances on the device between graph replays)
 		int debugEncLayers = -1;

@@ -137,6 +137,23 @@ namespace kern
 
 	// row-wise softmax of [rows][n] (all-logits test mode)
 	cudaError_t softmaxRows( const float* logits, float* probs, int rows, int n, cudaStream_t s );
+
+	// whisper_lang_auto_detect's choice for every row of a batch (whisper.cpp:2428-2495), after the [sot] pass and softmaxRows: the
+	// language tokens' probabilities probs[b][tokLang0 + l], l < nLangs, ordered descending (equal values: lower l first), exp() of
+	// each summed in that order in f32, langProbs[b][l] = exp(p_l) / sum, langIds[b] = the top l.  Row b's prompt is then written to
+	// tokens[b * nPrompt + i]: tmpl[i], with tmpl[autoPos] replaced by tokLang0 + langIds[b].
+	constexpr int kLangPromptMax = 256;
+	struct LangPickArgs
+	{
+		const float* probs = nullptr;   // [B][nVocab]
+		int nVocab = 0, tokLang0 = 0, nLangs = 0;
+		int* langIds = nullptr;         // [B]
+		float* langProbs = nullptr;     // [B][nLangs]
+		int* tokens = nullptr;          // [B][nPrompt]
+		int nPrompt = 0, autoPos = 0;
+		int tmpl[ kLangPromptMax ];
+	};
+	cudaError_t langPick( const LangPickArgs& a, int B, cudaStream_t s );
 	// one-time function attributes (dynamic shared memory opt-in) so that nothing but launches happens under stream capture
 	cudaError_t prepare( int maxK );
 

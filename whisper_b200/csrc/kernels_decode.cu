@@ -710,6 +710,54 @@ namespace kern
 		return cudaGetLastError();
 	}
 
+	// one CTA per row; the rank of each language is counted against all others, so the descending order (and the f32 sum taken in it)
+	// is the reference's whatever the thread count
+	constexpr int LP_THREADS = 128;
+	__global__ void __launch_bounds__( LP_THREADS )
+		lang_pick_kernel( const LangPickArgs a )
+	{
+		extern __shared__ float langSh[];
+		float* val = langSh;              // [nLangs] the row's language probabilities, by language
+		float* ord = langSh + a.nLangs;   // [nLangs] the same values, descending
+		__shared__ float sum;
+		__shared__ int top;
+		const int b = blockIdx.x, n = a.nLangs, tid = threadIdx.x;
+		const float* row = a.probs + (size_t)b * a.nVocab + a.tokLang0;
+		// a NaN counts as the lowest value, so the ranks below are a permutation whatever the row holds
+		for( int i = tid; i < n; i += LP_THREADS ) { const float p = row[ i ]; val[ i ] = isnan( p ) ? -INFINITY : p; }
+		__syncthreads();
+		for( int i = tid; i < n; i += LP_THREADS )
+		{
+			const float v = val[ i ];
+			int r = 0;
+			for( int j = 0; j < n; j++ )
+			{
+				const float w = val[ j ];
+				r += ( w > v || ( w == v && j < i ) ) ? 1 : 0;   // stable: a tie goes to the lower id, as wsp_detect_language's stable_sort
+			}
+			ord[ r ] = v;
+			if( r == 0 ) top = i;
+		}
+		__syncthreads();
+		if( tid == 0 )
+		{
+			float s = 0;
+			for( int k = 0; k < n; k++ ) s += (float)exp( (double)ord[ k ] );
+			sum = s;
+			a.langIds[ b ] = top;
+		}
+		__syncthreads();
+		for( int i = tid; i < n; i += LP_THREADS ) a.langProbs[ (size_t)b * n + i ] = (float)( exp( (double)val[ i ] ) / (double)sum );
+		for( int i = tid; i < a.nPrompt; i += LP_THREADS )
+			a.tokens[ (size_t)b * a.nPrompt + i ] = i == a.autoPos ? a.tokLang0 + top : a.tmpl[ i ];
+	}
+	cudaError_t langPick( const LangPickArgs& a, int B, cudaStream_t s )
+	{
+		if( a.nLangs < 1 || a.nPrompt < 1 || a.nPrompt > kLangPromptMax || a.autoPos < 0 || a.autoPos >= a.nPrompt ) return cudaErrorInvalidValue;
+		lang_pick_kernel<<<B, LP_THREADS, (size_t)2 * a.nLangs * sizeof( float ), s>>>( a );
+		return cudaGetLastError();
+	}
+
 	__global__ void advance_kernel( int* dNPast, int N, int* dForceTs, int* dStep, const int* nEnded, volatile int* nEndedHost )
 	{
 		ptx::pdl_launch_dependents();
