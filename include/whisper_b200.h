@@ -20,6 +20,8 @@
  *   wsp_run_chunks            the fixed-length greedy chunk loop of BASELINE.md §2 (mel + encode + n_decode x (decode + sample))
  *   wsp_run_chunks_until_eot  the same loop, each chunk cut at its first EOT and the batch stopped soon after its last one
  *   wsp_get_chunk_languages   whisper_lang_auto_detect (Whisper/source/whisper.cpp:2428-2495) per chunk of a run_chunks* call
+ *   wsp_run_chunks_window     the same loop, each chunk decoded and ended as whisper_full's first window (whisper.cpp:2910-3003)
+ *   wsp_window_segments       whisper_full's segments of one window (whisper.cpp:3026-3119)
  *   wsp_get_tensor            the reference's named trace points, Whisper/Utils/Trace/tracing.h (names as in whisper.cpp:1121-1869)
  *
  * Error handling mirrors the reference's HRESULT convention (SURVEY.md §8b): every function returns a wsp_status that the COM
@@ -183,7 +185,7 @@ wsp_status wsp_run_chunks_resident( wsp_context* c, int32_t batch, const int32_t
 /* The batch path of wsp_run_chunks, ending each chunk at its first EOT: chunk b's output is its greedy tokens up to and including
  * the first EOT, or max_decode tokens if it samples none; n_out[b] = that count; tokens_out[b*max_decode + i] for i < n_out[b]
  * (tokens_out may be NULL; entries past n_out[b] are not written).  EOT and max_decode are the only stop rules: whisper_full's others
- * (a timestamp past the window's end, max_tokens) do not apply.  A chunk that has ended stays in the batch and keeps being decoded
+ * (a timestamp past the window's end, max_tokens) do not apply here; wsp_run_chunks_window applies them.  A chunk that has ended stays in the batch and keeps being decoded
  * until the batch stops; its later tokens are not part of its output.  The steps go out in blocks of 8 and the host reads the
  * number of ended chunks one block behind, so the batch stops at most 16 steps after its last chunk's EOT.
  * pcm == NULL runs from the slots' resident PCM (wsp_upload_pcm), as wsp_run_chunks_resident does; otherwise n_samples is required.
@@ -197,6 +199,52 @@ wsp_status wsp_run_chunks_until_eot( wsp_context* c, const float* const* pcm, co
  * WSP_S_FALSE, writing nothing, when that call had no sentinel (or there was none); WSP_E_BOUNDS for a batch above that call's or a
  * short cap_floats. */
 wsp_status wsp_get_chunk_languages( wsp_context* c, int32_t batch, int32_t* lang_ids, float* lang_probs, size_t cap_floats );
+
+/* ---- whisper_full's first window on the batch path ---- */
+typedef struct wsp_window_params
+{
+	int32_t max_tokens;       /* whisper_full_params::max_tokens: a segment ends after token max_tokens (<= 0: no limit) */
+	int32_t single_segment;   /* whisper_full_params::single_segment */
+} wsp_window_params;
+typedef struct wsp_window_result
+{
+	int32_t n_sampled;        /* tokens the window sampled, a token that went back in time included */
+	int32_t n_tokens;         /* result_len: the first n_tokens of them are the window's result */
+	int32_t seek_delta;       /* frames the window advances by */
+	int32_t failed;           /* no usable timestamp (whisper.cpp:2977, 3000-3003): whisper_full drops the window */
+} wsp_window_result;
+/* The batch path of wsp_run_chunks, with each chunk decoded as whisper_full decodes its first window (Whisper/source/whisper.cpp:
+ * 2910-3003): a window at seek 0 over the chunk's n_len = wsp_mel_len frames (n_samples / 160, or / 320 under speed-up), ended by
+ * EOT, by max_tokens, by a timestamp at or past n_len - 100 frames, by a timestamp that goes back in time, or after n_max =
+ * n_text_ctx / 2 - 4 tokens, where it fails unless it holds a timestamp of at least 15 s.  Every chunk keeps the one caller prompt,
+ * as whisper_full's first window does with no prompt past.  Chunk b's tokens with their probabilities go to tokens_out[b*cap + i]
+ * for i < results[b].n_sampled (tokens_out may be NULL; cap >= n_max, else WSP_E_BOUNDS).  A chunk of at most 100 frames runs no
+ * window (whisper.cpp:2871): its result is all zeros.  The batch never runs more than n_max steps and stops at most 16 steps after
+ * its last window ends.  pcm == NULL runs from the slots' resident PCM; the prompt may hold WSP_TOKEN_LANGUAGE_AUTO; audio_ctx and
+ * speed-up apply as they do to wsp_run_chunks.  Every argument is checked before anything is enqueued; stage_ms as in
+ * wsp_run_chunks_until_eot. */
+wsp_status wsp_run_chunks_window( wsp_context* c, const float* const* pcm, const int32_t* n_samples, int32_t batch, const int32_t* prompt,
+	int32_t n_prompt, const wsp_window_params* params, wsp_token_data* tokens_out, int32_t cap, wsp_window_result* results, float* stage_ms );
+
+/* segmentation flags */
+enum
+{
+	WSP_SEGMENT_SINGLE = 1,          /* whisper_full_params::single_segment: timestamps do not split */
+	WSP_SEGMENT_PRINT_SPECIAL = 2,   /* print_special: special tokens count as text */
+	WSP_SEGMENT_SPEED_UP = 4,        /* speed_up: times are doubled (whisper.cpp:3044, 3088) */
+};
+typedef struct wsp_segment
+{
+	int64_t t0, t1;           /* 10 ms units */
+	int32_t i0, i1;           /* the segment's tokens are [i0, i1) of the window's */
+} wsp_segment;
+/* Host only: whisper_full's segments of one window at `seek` (whisper.cpp:3026-3119), from its result and its first result->n_tokens
+ * tokens.  A timestamp token closes a segment unless single-segment; consecutive timestamps are skipped, and a segment is emitted only
+ * if its text is not empty.  A segment's text is the text of its tokens [i0, i1), special tokens (id >= eot) left out unless
+ * WSP_SEGMENT_PRINT_SPECIAL.  A failed window has none.  *n_segs = the number of segments; the first min(*n_segs, cap) are written
+ * (segs may be NULL when cap is 0), and more than cap is WSP_E_BOUNDS.  n_tokens + 1 always suffices. */
+wsp_status wsp_window_segments( const wsp_model* m, const wsp_token_data* tokens, const wsp_window_result* result, int32_t seek,
+	uint32_t flags, wsp_segment* segs, int32_t cap, int32_t* n_segs );
 
 /* ---- several devices in one process (csrc/replicas.cpp) ----
  * Chunks are independent (SURVEY.md §8e): one engine + context per listed device (a device may be listed twice: two contexts on one
@@ -277,6 +325,10 @@ wsp_status wsp_test_skinny( int32_t device, int32_t nOut, int32_t K, int32_t col
  * the rules of whisper_sample_best / whisper_sample_timestamp (whisper.cpp:1875-1964); special4 = { beg, sot, solm, not } */
 wsp_status wsp_test_sample( int32_t device, int32_t rows, int32_t n_vocab, const float* logits, const int32_t special4[ 4 ], int32_t force_timestamp,
 	int32_t is_initial, float* probs, wsp_token_data* out );
+/* host only: whisper_full's window rule (csrc/window_rule.h, the code runFull and the sampler epilogue run) over ids[n] from step 0 of
+ * a window at `seek` over seek_end frames; rule4 = { eot, beg, max_tokens, single_segment }, n_max = n_text_ctx / 2 - 4.  out5 =
+ * { has_ts, seek_delta, result_len, failed, ended }; *n_steps = the tokens it consumed (the one that ended the window included). */
+wsp_status wsp_test_window_rule( const int32_t rule4[ 4 ], int32_t n_max, int32_t seek, int32_t seek_end, const int32_t* ids, int32_t n, int32_t out5[ 5 ], int32_t* n_steps );
 /* LayerNorm rows x d f32 -> f16 bit patterns */
 wsp_status wsp_test_layernorm( int32_t device, int32_t rows, int32_t d, const float* x, const float* gamma, const float* beta, uint16_t* out );
 

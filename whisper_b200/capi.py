@@ -27,6 +27,23 @@ class TokenData(C.Structure):
     _fields_ = [("id", C.c_int32), ("tid", C.c_int32), ("p", C.c_float), ("pt", C.c_float), ("ptsum", C.c_float)]
 
 
+class WindowParams(C.Structure):
+    _fields_ = [("max_tokens", C.c_int32), ("single_segment", C.c_int32)]
+
+
+class WindowResult(C.Structure):
+    _fields_ = [("n_sampled", C.c_int32), ("n_tokens", C.c_int32), ("seek_delta", C.c_int32), ("failed", C.c_int32)]
+
+
+class Segment(C.Structure):
+    _fields_ = [("t0", C.c_int64), ("t1", C.c_int64), ("i0", C.c_int32), ("i1", C.c_int32)]
+
+
+SEGMENT_SINGLE = 1          # wsp_window_segments flags
+SEGMENT_PRINT_SPECIAL = 2
+SEGMENT_SPEED_UP = 4
+
+
 class ReplicaStats(C.Structure):
     _fields_ = [("device", C.c_int32), ("batches_done", C.c_int32), ("chunks_done", C.c_int32), ("failed", C.c_int32), ("busy_ms", C.c_float), ("load_ms", C.c_float)]
 
@@ -39,10 +56,10 @@ EXPORTS = [
     "wsp_engine_create", "wsp_engine_create_from_image", "wsp_engine_destroy", "wsp_engine_weight_bytes",
     "wsp_context_create", "wsp_context_destroy", "wsp_synchronize",
     "wsp_context_device_bytes", "wsp_pcm_to_mel", "wsp_pcm_to_mel_window", "wsp_set_mel", "wsp_mel_len", "wsp_get_mel", "wsp_encode", "wsp_set_audio_ctx", "wsp_set_speed_up", "wsp_decode", "wsp_get_logits", "wsp_get_probs",
-    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_run_chunks_until_eot", "wsp_get_chunk_languages", "wsp_upload_pcm", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
+    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_run_chunks_until_eot", "wsp_get_chunk_languages", "wsp_run_chunks_window", "wsp_window_segments", "wsp_upload_pcm", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
     "wsp_host_alloc", "wsp_host_free", "wsp_timings",
     "wsp_replicas_create", "wsp_replicas_count", "wsp_replicas_run_chunks", "wsp_replicas_debug_fail_next", "wsp_replicas_destroy",
-    "wsp_test_gemm", "wsp_test_attention", "wsp_test_skinny", "wsp_test_layernorm", "wsp_test_sample",
+    "wsp_test_gemm", "wsp_test_attention", "wsp_test_skinny", "wsp_test_layernorm", "wsp_test_sample", "wsp_test_window_rule",
 ]
 
 _lib = None
@@ -106,6 +123,10 @@ def lib():
     sig("wsp_run_chunks_resident", i32, [vp, i32, ip, i32, i32, ip, fp])
     sig("wsp_run_chunks_until_eot", i32, [vp, C.POINTER(fp), ip, i32, ip, i32, i32, ip, ip, fp])
     sig("wsp_get_chunk_languages", i32, [vp, i32, ip, fp, sz])
+    sig("wsp_run_chunks_window", i32, [vp, C.POINTER(fp), ip, i32, ip, i32, C.POINTER(WindowParams), C.POINTER(TokenData), i32,
+                                       C.POINTER(WindowResult), fp])
+    sig("wsp_window_segments", i32, [vp, C.POINTER(TokenData), C.POINTER(WindowResult), i32, u32, C.POINTER(Segment), i32, ip])
+    sig("wsp_test_window_rule", i32, [ip, i32, i32, i32, ip, i32, ip, ip])
     sig("wsp_upload_pcm", i32, [vp, i32, fp, i32])
     sig("wsp_timer_start", i32, [vp])
     sig("wsp_timer_stop", i32, [vp, fp])
@@ -193,6 +214,24 @@ class Model:
         p = self.L.wsp_model_file_data(self.h, C.byref(n))
         return p, n.value
 
+    def window_segments(self, tokens, result: dict, seek: int = 0, flags: int = 0):
+        """whisper_full's segments of one window (wsp_window_segments): tokens = list of token dicts (at least result["n_tokens"]),
+        result = the window's result dict.  Returns [dict(t0, t1, i0, i1, text)], times in 10 ms units; the text follows the
+        reference's rule (special tokens, id >= eot, only with SEGMENT_PRINT_SPECIAL)."""
+        n = max(len(tokens), 1)
+        td = (TokenData * n)(*[TokenData(t["id"], t["tid"], t["p"], t["pt"], t["ptsum"]) for t in tokens])
+        res = WindowResult(result["n_sampled"], result["n_tokens"], result["seek_delta"], result["failed"])
+        segs = (Segment * (result["n_tokens"] + 1))()
+        n_segs = np.zeros(1, np.int32)
+        check(self.L.wsp_window_segments(self.h, td, C.byref(res), seek, flags, segs, len(segs), _i(n_segs)))
+        eot = self.special["eot"]
+        out = []
+        for s in segs[:int(n_segs[0])]:
+            ids = [tokens[i]["id"] for i in range(s.i0, s.i1)]
+            text = "".join(self.token_text(i) or "" for i in ids if (flags & SEGMENT_PRINT_SPECIAL) or i < eot)
+            out.append(dict(t0=int(s.t0), t1=int(s.t1), i0=int(s.i0), i1=int(s.i1), text=text))
+        return out
+
     def token_text(self, i: int):
         t = self.L.wsp_model_token_text(self.h, i)
         return None if t is None else t.decode(errors="replace")
@@ -242,6 +281,7 @@ class Context:
         self.engine = engine
         self.model = engine.model
         self.max_batch = max_batch
+        self.speed_up = False
         h = C.c_void_p()
         check(self.L.wsp_context_create(engine.h, max_batch, C.byref(h)))
         self.h = h
@@ -287,6 +327,7 @@ class Context:
         """whisper_full_params::speed_up: whole-clip log-mels (pcm_to_mel, run_chunks*) through the reference's 2x phase vocoder,
         n_samples // 320 frames, so a 3000-frame window holds 60 s of audio.  Takes 0 or 1 (bools are accepted)."""
         check(self.L.wsp_set_speed_up(self.h, int(on)))
+        self.speed_up = bool(on)
 
     def decode(self, tokens, n_past: int, batch: int = 1, flags: int = 0):
         """tokens: [batch][n_tokens] (or None with DECODE_DEVICE_TOKENS).  Returns list of sampled dicts (or None)."""
@@ -353,6 +394,35 @@ class Context:
         st = np.zeros(3, np.float32)
         check(self.L.wsp_run_chunks_until_eot(self.h, ptrs, None if ns is None else _i(ns), batch, _i(pr), pr.size, max_decode, _i(toks), _i(n_out), _f(st)))
         return [toks[b, :n_out[b]].copy() for b in range(batch)], st
+
+    def run_chunks_window(self, pcms, prompt, max_tokens: int = 0, single_segment: bool = False, print_special: bool = False,
+                          batch: int | None = None):
+        """Each chunk decoded as whisper_full's first window (wsp_run_chunks_window).  pcms: list of float32 arrays, or None to run
+        `batch` chunks from the slots' resident PCM (upload_pcm).  Returns (list per chunk of dict(tokens=[token dicts], result=dict,
+        segments=[dict(t0, t1, i0, i1, text)]), stage_ms[3]); segment times are doubled while speed-up is on."""
+        ptrs, ns = None, None
+        if pcms is not None:
+            batch = len(pcms)
+            arrs = [np.ascontiguousarray(p, np.float32) for p in pcms]
+            ptrs = (C.POINTER(C.c_float) * batch)(*[_f(a) for a in arrs])
+            ns = np.array([a.size for a in arrs], np.int32)
+        pr = np.ascontiguousarray(prompt, np.int32)
+        cap = self.model.n_text_ctx // 2 - 4
+        toks = (TokenData * (batch * cap))()
+        res = (WindowResult * batch)()
+        st = np.zeros(3, np.float32)
+        prm = WindowParams(int(max_tokens), int(bool(single_segment)))
+        check(self.L.wsp_run_chunks_window(self.h, ptrs, None if ns is None else _i(ns), batch, _i(pr), pr.size, C.byref(prm), toks, cap,
+                                           res, _f(st)))
+        flags = ((SEGMENT_SINGLE if single_segment else 0) | (SEGMENT_PRINT_SPECIAL if print_special else 0)
+                 | (SEGMENT_SPEED_UP if self.speed_up else 0))
+        out = []
+        for b in range(batch):
+            r = res[b]
+            result = dict(n_sampled=r.n_sampled, n_tokens=r.n_tokens, seek_delta=r.seek_delta, failed=r.failed)
+            tk = [dict(id=t.id, tid=t.tid, p=t.p, pt=t.pt, ptsum=t.ptsum) for t in toks[b * cap:b * cap + r.n_sampled]]
+            out.append(dict(tokens=tk, result=result, segments=self.model.window_segments(tk, result, 0, flags)))
+        return out, st
 
     def chunk_languages(self, batch: int):
         """The languages the last run_chunks* call detected for chunks [0, batch) (its prompt held TOKEN_LANGUAGE_AUTO): (ids[batch],
@@ -460,6 +530,18 @@ def test_skinny(W16, X16, iters: int = 0, device: int = 0):
     ms = C.c_float(0)
     check(lib().wsp_test_skinny(device, nOut, K, cols, _u16(W16.view(np.uint16)), _u16(X16.view(np.uint16)), _f(out), iters, C.byref(ms)))
     return out, ms.value
+
+
+def test_window_rule(ids, eot: int, beg: int, max_tokens: int = 0, single_segment: bool = False, n_max: int = 220, seek: int = 0,
+                     seek_end: int = 3000):
+    """csrc/window_rule.h on the host over a token sequence from step 0 -> (dict(has_ts, seek_delta, result_len, failed, ended),
+    tokens consumed)"""
+    a = np.ascontiguousarray(ids, np.int32)
+    rule = np.array([eot, beg, max_tokens, int(bool(single_segment))], np.int32)
+    out = np.zeros(5, np.int32)
+    n = np.zeros(1, np.int32)
+    check(lib().wsp_test_window_rule(_i(rule), n_max, seek, seek_end, _i(a), a.size, _i(out), _i(n)))
+    return dict(zip(["has_ts", "seek_delta", "result_len", "failed", "ended"], [int(x) for x in out])), int(n[0])
 
 
 def test_layernorm(x, gamma, beta, device: int = 0):

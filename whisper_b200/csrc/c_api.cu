@@ -268,6 +268,63 @@ wsp_status wsp_get_chunk_languages( wsp_context* c, int32_t batch, int32_t* lang
 	if( lang_probs ) std::copy( cx.lastLangProbs.begin(), cx.lastLangProbs.begin() + (size_t)batch * nLangs, lang_probs );
 	return WSP_OK;
 }
+wsp_status wsp_run_chunks_window( wsp_context* c, const float* const* pcm, const int32_t* n_samples, int32_t batch, const int32_t* prompt,
+	int32_t n_prompt, const wsp_window_params* params, wsp_token_data* tokens_out, int32_t cap, wsp_window_result* results, float* stage_ms )
+{
+	if( !c ) return fail( WSP_E_POINTER, "context" );
+	if( !params || !results ) return fail( WSP_E_POINTER, "params/results" );
+	if( pcm && !n_samples ) return fail( WSP_E_POINTER, "n_samples" );
+	return guarded( [ & ]() -> wsp_status {
+		const WindowOut w{ *params, tokens_out, cap, results };
+		const int nMax = c->c->e->hp.n_text_ctx / 2 - 4;                                             // whisper.cpp:2926
+		return ctxRunChunks( *c->c, pcm, n_samples, batch, prompt, n_prompt, nMax, nullptr, nullptr, stage_ms, pcm == nullptr, &w );
+	} );
+}
+wsp_status wsp_window_segments( const wsp_model* m, const wsp_token_data* tokens, const wsp_window_result* result, int32_t seek,
+	uint32_t flags, wsp_segment* segs, int32_t cap, int32_t* n_segs )
+{
+	if( !m || !result || !n_segs || ( cap > 0 && !segs ) ) return fail( WSP_E_POINTER, "model/result/segs/n_segs" );
+	if( cap < 0 || result->n_tokens < 0 || result->n_tokens > result->n_sampled ) return fail( WSP_E_INVALIDARG, "cap/result" );
+	const int len = result->failed ? 0 : result->n_tokens;
+	if( len > 0 && !tokens ) return fail( WSP_E_POINTER, "tokens" );
+	const int eot = m->m->vocab.token_eot, beg = m->m->vocab.token_beg;
+	const bool single = ( flags & WSP_SEGMENT_SINGLE ) != 0, special = ( flags & WSP_SEGMENT_PRINT_SPECIAL ) != 0;
+	const int64_t scale = ( flags & WSP_SEGMENT_SPEED_UP ) ? 2 : 1;
+	int n = 0;
+	auto emit = [ & ]( int64_t t0, int64_t t1, int i0, int i1 ) {
+		if( n < cap ) segs[ n ] = wsp_segment{ scale * t0, scale * t1, i0, i1 };
+		n++;
+	};
+	// whisper.cpp:3026-3119, with `text` reduced to whether it is empty: a segment's text is that of its tokens [i0, i1)
+	if( len > 0 )
+	{
+		int i0 = 0;
+		int64_t t0 = seek + 2 * ( (int64_t)tokens[ 0 ].tid - beg );
+		bool text = false;
+		for( int i = 0; i < len; i++ )
+		{
+			const int id = tokens[ i ].id;
+			if( special || id < eot )
+			{
+				const char* t = wsp_model_token_text( m, id );
+				if( t && *t ) text = true;
+			}
+			if( id > beg && !single )
+			{
+				const int64_t t1 = seek + 2 * ( (int64_t)tokens[ i ].tid - beg );
+				if( text ) emit( t0, t1, i0, i + 1 );
+				text = false;
+				while( i < len && tokens[ i ].id > beg ) i++;
+				i--;
+				t0 = t1;
+				i0 = i + 1;
+			}
+		}
+		if( text ) emit( t0, (int64_t)seek + result->seek_delta, i0, len );
+	}
+	*n_segs = n;
+	return n > cap ? fail( WSP_E_BOUNDS, "more segments than cap" ) : WSP_OK;
+}
 
 wsp_status wsp_upload_pcm( wsp_context* c, int32_t slot, const float* pcm, int32_t n_samples )
 {
@@ -618,6 +675,19 @@ wsp_status wsp_test_skinny( int32_t device, int32_t nOut, int32_t K, int32_t col
 	}
 	g_launchCount.fetch_add( (uint64_t)( 1 + ( iters > 0 ? iters : 0 ) ) );
 	WSP_CUDA( cudaMemcpy( out, dO.p, (size_t)cols * nOut * 4, cudaMemcpyDeviceToHost ) );
+	return WSP_OK;
+}
+
+wsp_status wsp_test_window_rule( const int32_t rule4[ 4 ], int32_t n_max, int32_t seek, int32_t seek_end, const int32_t* ids, int32_t n, int32_t out5[ 5 ], int32_t* n_steps )
+{
+	if( !rule4 || !out5 || !n_steps || ( n > 0 && !ids ) ) return fail( WSP_E_POINTER, "rule4/ids/out5/n_steps" );
+	const WindowRule r{ rule4[ 0 ], rule4[ 1 ], rule4[ 2 ], rule4[ 3 ], n_max };
+	WindowState s = windowStart();
+	int i = 0;
+	while( i < n && !windowStep( s, r, seek, seek_end, i, ids[ i ] ) ) i++;
+	*n_steps = i < n ? i + 1 : n;
+	const int32_t o[ 5 ] = { s.hasTs, s.seekDelta, s.resultLen, s.failed, s.ended };
+	memcpy( out5, o, sizeof( o ) );
 	return WSP_OK;
 }
 

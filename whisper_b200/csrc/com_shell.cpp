@@ -11,6 +11,7 @@
 #include "pcm_streamer.h"
 #include "capture_loop.h"
 #include "wav_reader.h"
+#include "window_rule.h"
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -1183,42 +1184,23 @@ namespace
 			}
 			prompt.insert( prompt.end(), promptInit.begin(), promptInit.end() );
 
-			int seekDelta = 100 * 30;                                                              // WHISPER_CHUNK_SIZE = 30
-			int resultLen = 0;
 			tokensCur.clear();
-			bool failed = false, hasTs = false;
-
-			const int nMax = nTextCtx / 2 - 4;                                                     // :2926
-			for( int i = 0; i < nMax; i++ )
+			const wsp::WindowRule rule{ tokEot, tokBeg, params.max_tokens, singleSegment ? 1 : 0, nTextCtx / 2 - 4 };   // :2926
+			wsp::WindowState win = wsp::windowStart();
+			for( int i = 0; i < rule.nMax && !win.ended; i++ )
 			{
 				wsp_token_data token;
 				HR( decode( prompt, nPast, i == 0, token ) );                                      // :2927-2943 decode + sample
 				nPast += (int)prompt.size();
 				prompt.clear();
-				if( token.id > tokBeg )                                                            // :2946-2957
-				{
-					const int seekDeltaNew = 2 * ( token.id - tokBeg );
-					if( hasTs && seekDelta > seekDeltaNew && resultLen < i ) break;
-					seekDelta = seekDeltaNew;
-					resultLen = i + 1;
-					hasTs = true;
-				}
 				prompt.push_back( token.id );
-				tokensCur.push_back( token );
-				if( token.id == tokEot || ( params.max_tokens > 0 && i >= params.max_tokens ) || ( hasTs && seek + seekDelta + 100 >= seekEnd ) )   // :2969-2988
-				{
-					if( resultLen == 0 )
-					{
-						if( seek + seekDelta + 100 >= seekEnd ) resultLen = i + 1;
-						else { failed = true; break; }
-					}
-					if( singleSegment ) { resultLen = i + 1; seekDelta = 100 * 30; }
-					break;
-				}
-				if( i == nMax - 1 && ( resultLen == 0 || seekDelta < 100 * 30 / 2 ) ) { failed = true; break; }   // :3000-3003
+				tokensCur.push_back( token );   // a token that goes back in time ends the window past its result: the resize drops it
+				wsp::windowStep( win, rule, seek, seekEnd, i, token.id );                           // :2946-3003
 			}
+			const int seekDelta = win.seekDelta, resultLen = win.resultLen;
+			const wsp_window_result result{ (int32_t)tokensCur.size(), resultLen, seekDelta, win.failed };
 
-			if( failed )                                                                           // :3006-3016
+			if( win.failed )                                                                       // :3006-3016
 			{
 				if( !promptPast.empty() ) promptPast.clear();
 				else
@@ -1252,31 +1234,21 @@ namespace
 				return S_OK;
 			};
 
-			if( !tokensCur.empty() )                                                               // :3026-3119
+			// :3026-3119
+			std::vector<wsp_segment> segs( tokensCur.size() + 1 );
+			int32_t nSegs = 0;
+			const uint32_t segFlags = ( singleSegment ? WSP_SEGMENT_SINGLE : 0 ) | ( printSpecial ? WSP_SEGMENT_PRINT_SPECIAL : 0 );
+			HR( check( wsp_window_segments( eng->model, tokensCur.data(), &result, seek, segFlags, segs.data(), (int32_t)segs.size(), &nSegs ), "wsp_window_segments" ) );
+			for( int k = 0; k < nSegs; k++ )
 			{
-				int i0 = 0;
-				int64_t t0 = seek + 2 * ( (int64_t)tokensCur.front().tid - tokBeg );
 				std::string text;
-				for( int i = 0; i < (int)tokensCur.size(); i++ )
+				for( int i = segs[ k ].i0; i < segs[ k ].i1; i++ )
 				{
 					const int id = tokensCur[ i ].id;
-					if( printSpecial || id < tokEot )
-					{
-						const char* t = wsp_model_token_text( eng->model, id );
-						if( t ) text += t;
-					}
-					if( id > tokBeg && !singleSegment )
-					{
-						const int64_t t1 = seek + 2 * ( (int64_t)tokensCur[ i ].tid - tokBeg );
-						if( !text.empty() ) HR( emit( t0, t1, text, i0, i + 1 ) );
-						text.clear();
-						while( i < (int)tokensCur.size() && tokensCur[ i ].id > tokBeg ) i++;
-						i--;
-						t0 = t1;
-						i0 = i + 1;
-					}
+					const char* t = printSpecial || id < tokEot ? wsp_model_token_text( eng->model, id ) : nullptr;
+					if( t ) text += t;
 				}
-				if( !text.empty() ) HR( emit( t0, (int64_t)seek + seekDelta, text, i0, (int)tokensCur.size() ) );
+				HR( emit( segs[ k ].t0, segs[ k ].t1, text, segs[ k ].i0, segs[ k ].i1 ) );
 			}
 			seek += seekDelta;                                                                     // :3121
 		}

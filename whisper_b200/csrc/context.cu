@@ -37,7 +37,7 @@ namespace wsp
 		for( auto& v : prof.pool ) cudaEventDestroy( v );
 		for( auto& v : timerEv ) if( v ) cudaEventDestroy( v );
 		void* bufs[] = { stepLayers, flowBias, flowExch, flowCtrl, megaBarrier, stepMarks, melMax, pcmDev, melF16, conv1, x, xn, q, k, vt, attn, h, crossK, crossV, selfK, selfV, xd, qd, attnD, hD, logits, probs, tieScratch,
-			tokensDev, dNPast, sampled, history, endStep, langIds, langProbs };
+			tokensDev, dNPast, sampled, history, endStep, langIds, langProbs, winCtl, winState, tokenLog };
 		for( void* b : bufs ) if( b ) cudaFree( b );
 		if( nEndedHost ) cudaFreeHost( nEndedHost );
 		for( auto& v : ev ) if( v ) cudaEventDestroy( v );
@@ -97,6 +97,9 @@ namespace wsp
 		c.histCap = hp.n_text_ctx;
 		WSP_CHECK( devAlloc( c.history, B * c.histCap, true ) );
 		WSP_CHECK( devAlloc( c.endStep, B, true ) );
+		WSP_CHECK( devAlloc( c.winCtl, 4 + B, true ) );
+		WSP_CHECK( devAlloc( c.winState, B, true ) );
+		WSP_CHECK( devAlloc( c.tokenLog, B * c.histCap, true ) );
 		if( e->nLangs > 0 )
 		{
 			WSP_CHECK( devAlloc( c.langIds, B, true ) );
@@ -489,7 +492,11 @@ namespace wsp
 		sa.tokenBeg = e.tokBeg; sa.tokenSot = e.tokSot; sa.tokenSolm = e.tokSolm; sa.tokenNot = e.tokNot;
 		sa.dForceTs = c.dFlags; sa.out = c.sampled; sa.nextTokens = c.tokensDev; sa.dNPast = c.dNPast; sa.N = N;
 		sa.history = c.history; sa.histCap = c.histCap; sa.dStep = c.dStep;
-		if( c.eotArmed ) { sa.tokenEot = e.tokEot; sa.endStep = c.endStep; sa.nEnded = c.nEnded; sa.nEndedHost = c.nEndedMapped; }
+		if( c.eotArmed )
+		{
+			sa.tokenEot = e.tokEot; sa.endStep = c.endStep; sa.nEnded = c.nEnded; sa.nEndedHost = c.nEndedMapped;
+			sa.winCtl = c.winCtl; sa.winState = c.winState; sa.tokenLog = c.tokenLog;
+		}
 		WSP_KERNEL( KK_OTHER, kern::sampleGreedy( sa, c.stream ) );
 		return WSP_OK;
 	}
@@ -738,7 +745,7 @@ namespace wsp
 	constexpr int kEotLag = 8;
 
 	int ctxRunChunks( Context& c, const float* const* pcm, const int32_t* nSamples, int batch, const int32_t* prompt, int nPrompt, int nDecode,
-		int32_t* tokensOut, int32_t* nOut, float* stageMs, bool resident )
+		int32_t* tokensOut, int32_t* nOut, float* stageMs, bool resident, const WindowOut* window )
 	{
 		const HParams& hp = c.e->hp;
 		if( batch < 1 || batch > c.maxB ) return fail( WSP_E_BOUNDS, "batch exceeds the context's max_batch" );
@@ -758,9 +765,16 @@ namespace wsp
 		if( detect && c.e->nLangs < 1 ) return fail( WSP_E_INVALIDARG, "WSP_TOKEN_LANGUAGE_AUTO needs a multilingual model" );
 		if( nDecode < 1 || nPrompt + nDecode > hp.n_text_ctx || nDecode > c.histCap ) return fail( WSP_E_BOUNDS, "n_prompt + n_decode exceeds n_text_ctx" );
 		if( !resident && ( !pcm || !nSamples ) ) return fail( WSP_E_POINTER, "pcm" );
-		if( !resident )
-			for( int b = 0; b < batch; b++ ) if( nSamples[ b ] < 0 ) return fail( WSP_E_INVALIDARG, "n_samples" );
+		for( int b = 0; b < batch; b++ )
+		{
+			if( !resident && nSamples[ b ] < 0 ) return fail( WSP_E_INVALIDARG, "n_samples" );
+			if( resident && !c.slots[ b ].pcm ) return fail( WSP_E_INVALIDARG, "no resident PCM in slot " + std::to_string( b ) + " (call wsp_upload_pcm)" );
+		}
 		const bool untilEot = nOut != nullptr;
+		if( window && window->cap < nDecode ) return fail( WSP_E_BOUNDS, "cap is below n_max" );
+		// each window runs at seek 0 over its chunk's mel length (whisper.cpp:2810-2818); one of at most 100 frames runs none (:2871)
+		std::vector<int32_t> seekEnd( window ? (size_t)batch : 0 );
+		for( size_t b = 0; b < seekEnd.size(); b++ ) seekEnd[ b ] = melFrames( c, resident ? c.slots[ b ].pcmSamples : nSamples[ b ] );
 		c.lastLangIds.clear();
 		c.lastLangProbs.clear();
 		WSP_CUDA( cudaSetDevice( c.e->device ) );
@@ -769,8 +783,6 @@ namespace wsp
 		if( resident )
 		{
 			// inputs already in HBM (wsp_upload_pcm): the log-mel front end still runs inside the timed region
-			for( int b = 0; b < batch; b++ )
-				if( !c.slots[ b ].pcm ) return fail( WSP_E_INVALIDARG, "no resident PCM in slot " + std::to_string( b ) + " (call wsp_upload_pcm)" );
 			WSP_CHECK( melBatchFromDevicePcm( c, 0, batch, [ & ]( int b ) { return (const float*)c.slots[ b ].pcm; }, [ & ]( int b ) { return c.slots[ b ].pcmSamples; } ) );
 		}
 		else
@@ -804,7 +816,7 @@ namespace wsp
 		launched( 3 );
 		if( detect ) WSP_CHECK( enqueueLanguageDetection( c, batch, prompt, nPrompt, autoPos ) );
 		int steps = nDecode;
-		if( !untilEot )
+		if( !untilEot && !window )
 		{
 			WSP_CHECK( decodeSubmit( c, nPrompt, batch, false, true ) );
 			for( int i = 1; i < nDecode; i++ )
@@ -812,12 +824,37 @@ namespace wsp
 		}
 		else
 		{
-			// the sampler logs every chunk's first EOT; the steps go out in blocks of kEotLag, and block k is enqueued before the host
-			// waits for block k - 1 and reads how many chunks have ended, so the stream never runs dry between blocks
+			// the sampler logs the step at which every chunk ends (its first EOT, or the window rule's end); the steps go out in blocks of
+			// kEotLag, and block k is enqueued before the host waits for block k - 1 and reads how many chunks have ended, so the stream
+			// never runs dry between blocks
 			struct Arm { Context& c; Arm( Context& x ) : c( x ) { c.eotArmed = true; } ~Arm() { c.eotArmed = false; } } arm( c );
 			*(volatile int*)c.nEndedHost = 0;
-			WSP_CUDA( cudaMemsetAsync( c.endStep, 0, (size_t)batch * 4, s ) );
-			WSP_CUDA( cudaMemsetAsync( c.nEnded, 0, 4, s ) );
+			if( !window )
+			{
+				WSP_CUDA( cudaMemsetAsync( c.endStep, 0, (size_t)batch * 4, s ) );
+				WSP_CUDA( cudaMemsetAsync( c.nEnded, 0, 4, s ) );
+				WSP_CUDA( cudaMemsetAsync( c.winCtl, 0, 4, s ) );
+			}
+			else
+			{
+				// a chunk too short for a window starts as ended (endStep -1) and counts as ended from the start
+				std::vector<int32_t> ctl( 4 + (size_t)batch ), ends( (size_t)batch, 0 );
+				std::vector<wsp::WindowState> st( (size_t)batch, wsp::windowStart() );
+				ctl[ 0 ] = 1; ctl[ 1 ] = window->params.max_tokens; ctl[ 2 ] = window->params.single_segment != 0; ctl[ 3 ] = nDecode;
+				int preEnded = 0;
+				for( int b = 0; b < batch; b++ )
+				{
+					ctl[ 4 + (size_t)b ] = seekEnd[ (size_t)b ];
+					if( seekEnd[ (size_t)b ] > 100 ) continue;
+					st[ (size_t)b ] = wsp::WindowState{ 0, 0, 0, 0, 1 };
+					ends[ (size_t)b ] = -1;
+					preEnded++;
+				}
+				WSP_CUDA( cudaMemcpyAsync( c.winCtl, ctl.data(), ctl.size() * 4, cudaMemcpyHostToDevice, s ) );
+				WSP_CUDA( cudaMemcpyAsync( c.winState, st.data(), st.size() * sizeof( wsp::WindowState ), cudaMemcpyHostToDevice, s ) );
+				WSP_CUDA( cudaMemcpyAsync( c.endStep, ends.data(), ends.size() * 4, cudaMemcpyHostToDevice, s ) );
+				WSP_CUDA( cudaMemcpyAsync( c.nEnded, &preEnded, 4, cudaMemcpyHostToDevice, s ) );
+			}
 			WSP_CHECK( decodeSubmit( c, nPrompt, batch, false, true ) );
 			steps = 1;
 			int waitOn = 0;
@@ -839,7 +876,14 @@ namespace wsp
 		// one D2H of the token log (and of the end-of-text steps) at the end: [batch][n_decode] int32
 		std::vector<int32_t> hist( (size_t)batch * c.histCap ), ends( (size_t)batch );
 		WSP_CUDA( cudaMemcpyAsync( hist.data(), c.history, hist.size() * 4, cudaMemcpyDeviceToHost, s ) );
-		if( untilEot ) WSP_CUDA( cudaMemcpyAsync( ends.data(), c.endStep, ends.size() * 4, cudaMemcpyDeviceToHost, s ) );
+		if( untilEot || window ) WSP_CUDA( cudaMemcpyAsync( ends.data(), c.endStep, ends.size() * 4, cudaMemcpyDeviceToHost, s ) );
+		std::vector<wsp::WindowState> winSt( window ? (size_t)batch : 0 );
+		std::vector<kern::TokenData> tdLog( window ? (size_t)batch * c.histCap : 0 );
+		if( window )
+		{
+			WSP_CUDA( cudaMemcpyAsync( winSt.data(), c.winState, winSt.size() * sizeof( wsp::WindowState ), cudaMemcpyDeviceToHost, s ) );
+			WSP_CUDA( cudaMemcpyAsync( tdLog.data(), c.tokenLog, tdLog.size() * sizeof( kern::TokenData ), cudaMemcpyDeviceToHost, s ) );
+		}
 		std::vector<int32_t> langIds( detect ? (size_t)batch : 0 );
 		std::vector<float> langProbs( detect ? (size_t)batch * c.e->nLangs : 0 );
 		if( detect )
@@ -850,6 +894,19 @@ namespace wsp
 		WSP_CUDA( cudaStreamSynchronize( s ) );
 		c.lastLangIds.swap( langIds );
 		c.lastLangProbs.swap( langProbs );
+		if( window )
+			for( int b = 0; b < batch; b++ )
+			{
+				const wsp::WindowState& st = winSt[ (size_t)b ];
+				const int n = ends[ (size_t)b ] > 0 ? ends[ (size_t)b ] : 0;
+				window->results[ b ] = wsp_window_result{ n, st.resultLen, st.seekDelta, st.failed };
+				if( window->tokens )
+					for( int i = 0; i < n; i++ )
+					{
+						const kern::TokenData& t = tdLog[ (size_t)b * c.histCap + i ];
+						window->tokens[ (size_t)b * window->cap + i ] = wsp_token_data{ t.id, t.tid, t.p, t.pt, t.ptsum };
+					}
+			}
 		for( int b = 0; b < batch; b++ )
 		{
 			const int n = untilEot && ends[ (size_t)b ] > 0 ? ends[ (size_t)b ] : nDecode;

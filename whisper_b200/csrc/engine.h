@@ -174,6 +174,10 @@ namespace wsp
 		int* nEndedHost = nullptr;      // mapped pinned copy of nEnded, written by the last kernel of every step
 		int* nEndedMapped = nullptr;    // its device address
 		cudaEvent_t blockEv[ 2 ] = { nullptr, nullptr };   // ends of the last two enqueued step blocks
+		// whisper_full's window rule of wsp_run_chunks_window, passed to the armed sampler of both calls; winCtl[0] = 0 (EOT) or 1 (rule)
+		int* winCtl = nullptr;          // [4 + maxB] on | max_tokens | single_segment | n_max, then each row's seek_end
+		wsp::WindowState* winState = nullptr;   // [maxB]
+		kern::TokenData* tokenLog = nullptr;    // [maxB][histCap] every armed step's TokenData
 		// per-chunk language detection of a run_chunks* call whose prompt holds WSP_TOKEN_LANGUAGE_AUTO (lang_pick_kernel)
 		int* langIds = nullptr;         // [maxB]
 		float* langProbs = nullptr;     // [maxB][nLangs]
@@ -233,7 +237,16 @@ namespace wsp
 	int ctxDecode( Context& c, const int32_t* tokensHost, int nTokens, int nPast, int batch, uint32_t flags, wsp_token_data* sampledHost );
 	int ctxUploadPcm( Context& c, int slot, const float* pcmHost, int nSamples );
 	int ctxProfileDecode( Context& c, int batch, int nSteps, float* msByKind, int* launchesByKind );
-	// nOut == nullptr: nDecode steps for every chunk (wsp_run_chunks*); else each chunk ends at its first EOT (wsp_run_chunks_until_eot)
+	// wsp_run_chunks_window's outputs
+	struct WindowOut
+	{
+		wsp_window_params params;
+		wsp_token_data* tokens;         // [batch][cap], may be null
+		int cap;
+		wsp_window_result* results;     // [batch]
+	};
+	// nOut == nullptr and window == nullptr: nDecode steps for every chunk (wsp_run_chunks*); nOut: each chunk ends at its first EOT
+	// (wsp_run_chunks_until_eot); window: each chunk ends by whisper_full's window rule, nDecode = n_max (wsp_run_chunks_window)
 	int ctxRunChunks( Context& c, const float* const* pcm, const int32_t* nSamples, int batch, const int32_t* prompt, int nPrompt, int nDecode,
-		int32_t* tokensOut, int32_t* nOut, float* stageMs, bool resident );
+		int32_t* tokensOut, int32_t* nOut, float* stageMs, bool resident, const WindowOut* window = nullptr );
 }

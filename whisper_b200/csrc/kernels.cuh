@@ -4,6 +4,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "window_rule.h"
 
 namespace kern
 {
@@ -131,6 +132,13 @@ namespace kern
 		int* endStep = nullptr;
 		int* nEnded = nullptr;
 		volatile int* nEndedHost = nullptr;
+		// armed callers also pass these (wsp_run_chunks_window): the step's TokenData goes to tokenLog[b][*dStep], and while
+		// winCtl[0] is set a row ends by whisper_full's window rule (window_rule.h) instead of at its first EOT.  winCtl = { on,
+		// max_tokens, single_segment, n_max }, then seekEnd[B]; winState[B] is the rows' state, and a row whose endStep the caller
+		// set non-zero never runs the rule
+		const int* winCtl = nullptr;
+		wsp::WindowState* winState = nullptr;
+		TokenData* tokenLog = nullptr;
 	};
 	// one cluster of 4 CTAs per row (any nVocab >= 8 whose quarter fits shared memory), then the 1-thread advance of n_past / flags / step
 	cudaError_t sampleGreedy( const SampleArgs& a, cudaStream_t s );

@@ -672,10 +672,22 @@ namespace kern
 			a.out[ b ] = td;
 			if( a.nextTokens ) a.nextTokens[ b ] = td.id;
 			if( a.history && a.dStep && *a.dStep < a.histCap ) a.history[ (size_t)b * a.histCap + *a.dStep ] = td.id;
-			if( a.endStep && td.id == a.tokenEot && a.endStep[ b ] == 0 )
+			if( a.tokenLog && a.dStep && *a.dStep < a.histCap ) a.tokenLog[ (size_t)b * a.histCap + *a.dStep ] = td;
+			if( a.endStep && a.endStep[ b ] == 0 )
 			{
-				a.endStep[ b ] = *a.dStep + 1;
-				atomicAdd( a.nEnded, 1 );
+				bool ended = td.id == a.tokenEot;
+				if( a.winCtl && a.winCtl[ 0 ] )
+				{
+					const wsp::WindowRule rule{ a.tokenEot, a.tokenBeg, a.winCtl[ 1 ], a.winCtl[ 2 ], a.winCtl[ 3 ] };
+					wsp::WindowState st = a.winState[ b ];
+					ended = wsp::windowStep( st, rule, 0, a.winCtl[ 4 + b ], *a.dStep, td.id );
+					a.winState[ b ] = st;
+				}
+				if( ended )
+				{
+					a.endStep[ b ] = *a.dStep + 1;
+					atomicAdd( a.nEnded, 1 );
+				}
 			}
 		}
 		}
