@@ -22,6 +22,9 @@
  *   wsp_get_chunk_languages   whisper_lang_auto_detect (Whisper/source/whisper.cpp:2428-2495) per chunk of a run_chunks* call
  *   wsp_run_chunks_window     the same loop, each chunk decoded and ended as whisper_full's first window (whisper.cpp:2910-3003)
  *   wsp_window_segments       whisper_full's segments of one window (whisper.cpp:3026-3119)
+ *   wsp_set_token_timestamps  whisper_full_params::token_timestamps (Whisper/API/sFullParams.h eFullParamsFlags::TokenTimestamps): the
+ *                             signal energy of get_signal_energy (whisper.cpp:3356-3372), computed on the device
+ *   wsp_window_token_times    those segments with whisper_full's token times (whisper.cpp:3374-3600) and max_len wrapping (:2713-2763)
  *   wsp_get_tensor            the reference's named trace points, Whisper/Utils/Trace/tracing.h (names as in whisper.cpp:1121-1869)
  *
  * Error handling mirrors the reference's HRESULT convention (SURVEY.md §8b): every function returns a wsp_status that the COM
@@ -246,6 +249,39 @@ typedef struct wsp_segment
 wsp_status wsp_window_segments( const wsp_model* m, const wsp_token_data* tokens, const wsp_window_result* result, int32_t seek,
 	uint32_t flags, wsp_segment* segs, int32_t cap, int32_t* n_segs );
 
+/* ---- token-level timestamps of whisper_full's first window on the batch path ---- */
+/* whisper_full_params::token_timestamps.  on = 1 makes the signal energy of get_signal_energy (whisper.cpp:3356-3372) context state:
+ * e[i] = (sum over j = -32..32 with 0 <= i + j < n of |x[i + j]|) / 65, summed in f32 in that order, bit-identical to the reference.
+ * While it is on, wsp_run_chunks_window computes it on the device for every chunk of its batch, from the PCM the call used (host or
+ * resident; under speed-up the original samples), right after the log-mel and inside stage_ms[0], and brings it back with the call's
+ * tokens; wsp_pcm_to_mel computes it for its slot.  wsp_get_tensor("energy", slot) returns it.  on = 0 (the default) changes nothing
+ * in any call; any other value is WSP_E_INVALIDARG. */
+wsp_status wsp_set_token_timestamps( wsp_context* c, int32_t on );
+typedef struct wsp_token_time
+{
+	int64_t t0, t1;           /* whisper_token_data::t0 / t1, 10 ms units; -1 for a token outside every segment */
+	float vlen;               /* whisper_token_data::vlen: voice length of the token's text */
+} wsp_token_time;
+typedef struct wsp_token_time_params
+{
+	float thold_pt;           /* whisper_full_params::thold_pt (default 0.01) */
+	float thold_ptsum;        /* whisper_full_params::thold_ptsum (default 0.01) */
+	int32_t max_len;          /* whisper_full_params::max_len: wrap segments at this many characters (<= 0: no wrapping) */
+} wsp_token_time_params;
+/* Host only: chunk `chunk`'s segments of this context's last wsp_run_chunks_window call as whisper_full emits them with
+ * token_timestamps on.  tokens and result are that call's for the chunk, flags as for wsp_window_segments.  The window is cut by
+ * wsp_window_segments; then, segment by segment in order and from the state whisper_full starts a call with, the token times of
+ * whisper.cpp:3374-3600 run over the chunk's signal energy, and with max_len > 0 each segment is wrapped right after its token
+ * times (:3063-3070, 3107-3114).  Under WSP_SEGMENT_SPEED_UP this is what the reference does: segment times are doubled, the
+ * timestamp token times t_beg + 2 (tid - beg) are not, and the energy is that of the original samples.  segs receives the segments
+ * after wrapping, the first min(*n_segs, cap) of them (a segment's text is that of its non-special tokens once wrapped);
+ * times[i] = window token i's times for i < result->n_tokens.  A failed window, or a chunk of at most 100 frames, has no segments.
+ * Errors, checked before anything is written: WSP_E_POINTER for a null pointer (tokens and times may be NULL only when the window
+ * has no result tokens), WSP_E_INVALIDARG when the last window call ran with the energy off or there was none, WSP_E_BOUNDS for a
+ * chunk outside that call's batch or, with *n_segs set, more segments than cap. */
+wsp_status wsp_window_token_times( wsp_context* c, int32_t chunk, const wsp_token_data* tokens, const wsp_window_result* result,
+	uint32_t flags, const wsp_token_time_params* p, wsp_segment* segs, int32_t cap, int32_t* n_segs, wsp_token_time* times );
+
 /* ---- several devices in one process (csrc/replicas.cpp) ----
  * Chunks are independent (SURVEY.md §8e): one engine + context per listed device (a device may be listed twice: two contexts on one
  * GPU), the model file read ONCE and its image copied device-to-device from devices[0] (cudaMemcpyPeer over NVLink) — the C++ form of
@@ -291,7 +327,8 @@ wsp_status wsp_profile_decode( wsp_context* c, int32_t batch, int32_t n_steps, f
  *   "enc.h"                [n][4d]      f16 MLP hidden gelu(LN2(x) W1^T + b1) of the last encoded layer
  *   "cross_k", "cross_v"   [L][H][n][64] f16 cross-attention memories (K scaled by 64^-0.25)
  *   "self_k", "self_v"     [L][H][n_text_ctx][64] f16 decoder self-KV cache (K scaled by 64^-0.25); row j = text position j
- *   "dec.x"                [8][d]       f32 decoder residual stream (shared by all slots) */
+ *   "dec.x"                [8][d]       f32 decoder residual stream (shared by all slots)
+ *   "energy"               [n_samples]  f32 signal energy of the chunk's PCM (wsp_set_token_timestamps); empty before any */
 wsp_status wsp_get_tensor( wsp_context* c, const char* name, int32_t slot, float* dst, size_t cap_floats, size_t* n_floats );
 /* debug: run only the first n encoder layers (negative = all) */
 wsp_status wsp_debug_set_encoder_layers( wsp_context* c, int32_t n );
@@ -329,6 +366,16 @@ wsp_status wsp_test_sample( int32_t device, int32_t rows, int32_t n_vocab, const
  * a window at `seek` over seek_end frames; rule4 = { eot, beg, max_tokens, single_segment }, n_max = n_text_ctx / 2 - 4.  out5 =
  * { has_ts, seek_delta, result_len, failed, ended }; *n_steps = the tokens it consumed (the one that ended the window included). */
 wsp_status wsp_test_window_rule( const int32_t rule4[ 4 ], int32_t n_max, int32_t seek, int32_t seek_end, const int32_t* ids, int32_t n, int32_t out5[ 5 ], int32_t* n_steps );
+/* host only: whisper_full's token times (csrc/token_times.h, the code runFull and wsp_window_token_times run) for one segment of
+ * tokens[n] over [t0, t1] with vlen[n], energy[n_samples] and the state state3 = { t_beg, t_last, tid_last } carried in and out;
+ * special2 = { beg, eot }; times[n] holds the times on entry (-1 where none) and on return.  WSP_S_FALSE, changing nothing, without
+ * energy (n_samples 0). */
+wsp_status wsp_test_token_times( const wsp_token_data* tokens, const float* vlen, int32_t n, int64_t t0, int64_t t1, const int32_t special2[ 2 ],
+	const float* energy, int32_t n_samples, float thold_pt, float thold_ptsum, int64_t state3[ 3 ], wsp_token_time* times );
+/* signal_energy_kernel alone over `batch` host clips pcm[b][n_samples[b]] -> energy[b][n_samples[b]] (host); with iters > 0, *ms = the
+ * mean time of one launch over `iters` more launches between CUDA events */
+wsp_status wsp_test_signal_energy( int32_t device, const float* const* pcm, const int32_t* n_samples, int32_t batch, float* const* energy,
+	int32_t iters, float* ms );
 /* LayerNorm rows x d f32 -> f16 bit patterns */
 wsp_status wsp_test_layernorm( int32_t device, int32_t rows, int32_t d, const float* x, const float* gamma, const float* beta, uint16_t* out );
 

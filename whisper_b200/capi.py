@@ -39,6 +39,14 @@ class Segment(C.Structure):
     _fields_ = [("t0", C.c_int64), ("t1", C.c_int64), ("i0", C.c_int32), ("i1", C.c_int32)]
 
 
+class TokenTime(C.Structure):
+    _fields_ = [("t0", C.c_int64), ("t1", C.c_int64), ("vlen", C.c_float)]
+
+
+class TokenTimeParams(C.Structure):
+    _fields_ = [("thold_pt", C.c_float), ("thold_ptsum", C.c_float), ("max_len", C.c_int32)]
+
+
 SEGMENT_SINGLE = 1          # wsp_window_segments flags
 SEGMENT_PRINT_SPECIAL = 2
 SEGMENT_SPEED_UP = 4
@@ -56,10 +64,10 @@ EXPORTS = [
     "wsp_engine_create", "wsp_engine_create_from_image", "wsp_engine_destroy", "wsp_engine_weight_bytes",
     "wsp_context_create", "wsp_context_destroy", "wsp_synchronize",
     "wsp_context_device_bytes", "wsp_pcm_to_mel", "wsp_pcm_to_mel_window", "wsp_set_mel", "wsp_mel_len", "wsp_get_mel", "wsp_encode", "wsp_set_audio_ctx", "wsp_set_speed_up", "wsp_decode", "wsp_get_logits", "wsp_get_probs",
-    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_run_chunks_until_eot", "wsp_get_chunk_languages", "wsp_run_chunks_window", "wsp_window_segments", "wsp_upload_pcm", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
+    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_run_chunks_until_eot", "wsp_get_chunk_languages", "wsp_run_chunks_window", "wsp_window_segments", "wsp_set_token_timestamps", "wsp_window_token_times", "wsp_upload_pcm", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
     "wsp_host_alloc", "wsp_host_free", "wsp_timings",
     "wsp_replicas_create", "wsp_replicas_count", "wsp_replicas_run_chunks", "wsp_replicas_debug_fail_next", "wsp_replicas_destroy",
-    "wsp_test_gemm", "wsp_test_attention", "wsp_test_skinny", "wsp_test_layernorm", "wsp_test_sample", "wsp_test_window_rule",
+    "wsp_test_gemm", "wsp_test_attention", "wsp_test_skinny", "wsp_test_layernorm", "wsp_test_sample", "wsp_test_window_rule", "wsp_test_token_times", "wsp_test_signal_energy",
 ]
 
 _lib = None
@@ -127,6 +135,12 @@ def lib():
                                        C.POINTER(WindowResult), fp])
     sig("wsp_window_segments", i32, [vp, C.POINTER(TokenData), C.POINTER(WindowResult), i32, u32, C.POINTER(Segment), i32, ip])
     sig("wsp_test_window_rule", i32, [ip, i32, i32, i32, ip, i32, ip, ip])
+    sig("wsp_set_token_timestamps", i32, [vp, i32])
+    sig("wsp_window_token_times", i32, [vp, i32, C.POINTER(TokenData), C.POINTER(WindowResult), u32, C.POINTER(TokenTimeParams),
+                                        C.POINTER(Segment), i32, ip, C.POINTER(TokenTime)])
+    sig("wsp_test_signal_energy", i32, [i32, C.POINTER(fp), ip, i32, C.POINTER(fp), i32, fp])
+    sig("wsp_test_token_times", i32, [C.POINTER(TokenData), fp, i32, C.c_int64, C.c_int64, ip, fp, i32, C.c_float, C.c_float,
+                                      C.POINTER(C.c_int64), C.POINTER(TokenTime)])
     sig("wsp_upload_pcm", i32, [vp, i32, fp, i32])
     sig("wsp_timer_start", i32, [vp])
     sig("wsp_timer_stop", i32, [vp, fp])
@@ -235,6 +249,9 @@ class Model:
     def token_text(self, i: int):
         t = self.L.wsp_model_token_text(self.h, i)
         return None if t is None else t.decode(errors="replace")
+
+    def token_bytes(self, i: int) -> bytes:
+        return self.L.wsp_model_token_text(self.h, i) or b""
 
     @property
     def multilingual(self):
@@ -395,11 +412,19 @@ class Context:
         check(self.L.wsp_run_chunks_until_eot(self.h, ptrs, None if ns is None else _i(ns), batch, _i(pr), pr.size, max_decode, _i(toks), _i(n_out), _f(st)))
         return [toks[b, :n_out[b]].copy() for b in range(batch)], st
 
+    def set_token_timestamps(self, on):
+        """whisper_full_params::token_timestamps: run_chunks_window and pcm_to_mel compute each chunk's signal energy on the device
+        (get_tensor("energy", b)), which run_chunks_window(token_times=...) needs.  Takes 0 or 1 (bools are accepted)."""
+        check(self.L.wsp_set_token_timestamps(self.h, int(on)))
+
     def run_chunks_window(self, pcms, prompt, max_tokens: int = 0, single_segment: bool = False, print_special: bool = False,
-                          batch: int | None = None):
+                          batch: int | None = None, token_times: dict | None = None):
         """Each chunk decoded as whisper_full's first window (wsp_run_chunks_window).  pcms: list of float32 arrays, or None to run
         `batch` chunks from the slots' resident PCM (upload_pcm).  Returns (list per chunk of dict(tokens=[token dicts], result=dict,
-        segments=[dict(t0, t1, i0, i1, text)]), stage_ms[3]); segment times are doubled while speed-up is on."""
+        segments=[dict(t0, t1, i0, i1, text)]), stage_ms[3]); segment times are doubled while speed-up is on.
+        token_times=dict(thold_pt=0.01, thold_ptsum=0.01, max_len=0) (token timestamps must be on): the segments are whisper_full's
+        with token_timestamps (wsp_window_token_times), wrapped at max_len characters when max_len > 0; the window's result tokens
+        then carry t0, t1 and vlen, and every segment holds its tokens as `tokens`."""
         ptrs, ns = None, None
         if pcms is not None:
             batch = len(pcms)
@@ -421,8 +446,38 @@ class Context:
             r = res[b]
             result = dict(n_sampled=r.n_sampled, n_tokens=r.n_tokens, seek_delta=r.seek_delta, failed=r.failed)
             tk = [dict(id=t.id, tid=t.tid, p=t.p, pt=t.pt, ptsum=t.ptsum) for t in toks[b * cap:b * cap + r.n_sampled]]
-            out.append(dict(tokens=tk, result=result, segments=self.model.window_segments(tk, result, 0, flags)))
+            if token_times is None:
+                segs = self.model.window_segments(tk, result, 0, flags)
+            else:
+                segs = self._token_times(b, toks, b * cap, res[b], tk, flags, print_special, token_times)
+            out.append(dict(tokens=tk, result=result, segments=segs))
         return out, st
+
+    def _token_times(self, b, toks, first, res, tk, flags, print_special, params):
+        p = dict(thold_pt=0.01, thold_ptsum=0.01, max_len=0)
+        p.update(params)
+        prm = TokenTimeParams(p["thold_pt"], p["thold_ptsum"], int(p["max_len"]))
+        n = res.n_tokens
+        times = (TokenTime * max(n, 1))()
+        n_segs = np.zeros(1, np.int32)
+        td = C.cast(C.byref(toks, first * C.sizeof(TokenData)), C.POINTER(TokenData))
+        st = self.L.wsp_window_token_times(self.h, b, td, C.byref(res), flags, C.byref(prm), None, 0, _i(n_segs), times)
+        if st != -7:                                     # WSP_E_BOUNDS: *n_segs holds the count
+            check(st)
+        segs = (Segment * max(int(n_segs[0]), 1))()
+        check(self.L.wsp_window_token_times(self.h, b, td, C.byref(res), flags, C.byref(prm), segs, len(segs), _i(n_segs), times))
+        for i in range(n):
+            tk[i].update(t0=int(times[i].t0), t1=int(times[i].t1), vlen=float(times[i].vlen))
+        eot = self.model.special["eot"]
+        out = []
+        for s in segs[:int(n_segs[0])]:
+            ids = [tk[i]["id"] for i in range(s.i0, s.i1)]
+            if p["max_len"] > 0:                         # a wrapped segment's text: its non-special tokens' bytes
+                text = b"".join(self.model.token_bytes(i) for i in ids if i < eot).decode(errors="replace")
+            else:                                        # as window_segments makes it
+                text = "".join(self.model.token_text(i) or "" for i in ids if print_special or i < eot)
+            out.append(dict(t0=int(s.t0), t1=int(s.t1), i0=int(s.i0), i1=int(s.i1), text=text, tokens=tk[s.i0:s.i1]))
+        return out
 
     def chunk_languages(self, batch: int):
         """The languages the last run_chunks* call detected for chunks [0, batch) (its prompt held TOKEN_LANGUAGE_AUTO): (ids[batch],
@@ -542,6 +597,34 @@ def test_window_rule(ids, eot: int, beg: int, max_tokens: int = 0, single_segmen
     n = np.zeros(1, np.int32)
     check(lib().wsp_test_window_rule(_i(rule), n_max, seek, seek_end, _i(a), a.size, _i(out), _i(n)))
     return dict(zip(["has_ts", "seek_delta", "result_len", "failed", "ended"], [int(x) for x in out])), int(n[0])
+
+
+def test_token_times(tokens, vlen, t0: int, t1: int, beg: int, eot: int, energy, thold_pt: float = 0.01, thold_ptsum: float = 0.01,
+                     state=(0, 0, 0), times=None):
+    """csrc/token_times.h on the host for one segment: tokens = dicts (id, tid, p, pt, ptsum), vlen = floats, energy = float32 array,
+    state = (t_beg, t_last, tid_last), times = [[t0, t1, vlen]] on entry (default all -1, 0).  -> (times as [[t0, t1, vlen]], state,
+    whether there was energy)"""
+    n = len(tokens)
+    td = (TokenData * max(n, 1))(*[TokenData(t["id"], t["tid"], t.get("p", 0.0), t["pt"], t["ptsum"]) for t in tokens])
+    vl = np.ascontiguousarray(vlen if n else [0.0], np.float32)
+    tt = (TokenTime * max(n, 1))(*[TokenTime(int(a), int(b_), float(v)) for a, b_, v in (times or [[-1, -1, 0.0]] * n)])
+    en = np.ascontiguousarray(energy if len(energy) else [0.0], np.float32)
+    st = (C.c_int64 * 3)(*[int(x) for x in state])
+    sp = np.array([beg, eot], np.int32)
+    rc = check(lib().wsp_test_token_times(td, _f(vl), n, t0, t1, _i(sp), _f(en), len(energy), thold_pt, thold_ptsum, st, tt))
+    return [[int(t.t0), int(t.t1), float(t.vlen)] for t in tt[:n]], [int(x) for x in st], rc == WSP_OK
+
+
+def test_signal_energy(pcms, iters: int = 0, device: int = 0):
+    """signal_energy_kernel alone over a batch of float32 clips -> (energies, ms of one launch averaged over iters launches)"""
+    arrs = [np.ascontiguousarray(p, np.float32) for p in pcms]
+    outs = [np.empty_like(a) for a in arrs]
+    ins = (C.POINTER(C.c_float) * len(arrs))(*[_f(a) for a in arrs])
+    dst = (C.POINTER(C.c_float) * len(arrs))(*[_f(o) for o in outs])
+    ns = np.array([a.size for a in arrs], np.int32)
+    ms = C.c_float(0)
+    check(lib().wsp_test_signal_energy(device, ins, _i(ns), len(arrs), dst, iters, C.byref(ms)))
+    return outs, ms.value
 
 
 def test_layernorm(x, gamma, beta, device: int = 0):

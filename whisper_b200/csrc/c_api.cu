@@ -1,6 +1,7 @@
 // extern "C" surface (include/whisper_b200.h) + kernel-level test hooks.
 #include "engine.h"
 #include "ref_arith.cuh"
+#include "token_times.h"
 #include <algorithm>
 #include <math.h>
 #include <math.h>
@@ -21,6 +22,51 @@ namespace
 		catch( const std::bad_alloc& ) { return fail( WSP_E_OUTOFMEMORY, "host allocation failed" ); }
 		catch( const std::exception& ex ) { return fail( WSP_E_INVALIDARG, ex.what() ); }
 		catch( ... ) { return fail( WSP_E_INVALIDARG, "unknown exception" ); }
+	}
+	// whisper_full's segments of one window (whisper.cpp:3026-3119), as wsp_window_segments documents them; textOf( id ) = the token's text
+	template<class T>
+	wsp_status windowSegments( T textOf, int eot, int beg, const wsp_token_data* tokens, const wsp_window_result* result, int32_t seek,
+		uint32_t flags, wsp_segment* segs, int32_t cap, int32_t* n_segs )
+	{
+		if( cap < 0 || result->n_tokens < 0 || result->n_tokens > result->n_sampled ) return fail( WSP_E_INVALIDARG, "cap/result" );
+		const int len = result->failed ? 0 : result->n_tokens;
+		if( len > 0 && !tokens ) return fail( WSP_E_POINTER, "tokens" );
+		const bool single = ( flags & WSP_SEGMENT_SINGLE ) != 0, special = ( flags & WSP_SEGMENT_PRINT_SPECIAL ) != 0;
+		const int64_t scale = ( flags & WSP_SEGMENT_SPEED_UP ) ? 2 : 1;
+		int n = 0;
+		auto emit = [ & ]( int64_t t0, int64_t t1, int i0, int i1 ) {
+			if( n < cap ) segs[ n ] = wsp_segment{ scale * t0, scale * t1, i0, i1 };
+			n++;
+		};
+		// with `text` reduced to whether it is empty: a segment's text is that of its tokens [i0, i1)
+		if( len > 0 )
+		{
+			int i0 = 0;
+			int64_t t0 = seek + 2 * ( (int64_t)tokens[ 0 ].tid - beg );
+			bool text = false;
+			for( int i = 0; i < len; i++ )
+			{
+				const int id = tokens[ i ].id;
+				if( special || id < eot )
+				{
+					const char* t = textOf( id );
+					if( t && *t ) text = true;
+				}
+				if( id > beg && !single )
+				{
+					const int64_t t1 = seek + 2 * ( (int64_t)tokens[ i ].tid - beg );
+					if( text ) emit( t0, t1, i0, i + 1 );
+					text = false;
+					while( i < len && tokens[ i ].id > beg ) i++;
+					i--;
+					t0 = t1;
+					i0 = i + 1;
+				}
+			}
+			if( text ) emit( t0, (int64_t)seek + result->seek_delta, i0, len );
+		}
+		*n_segs = n;
+		return n > cap ? fail( WSP_E_BOUNDS, "more segments than cap" ) : WSP_OK;
 	}
 	template<class T> struct DevTmp
 	{
@@ -284,46 +330,64 @@ wsp_status wsp_window_segments( const wsp_model* m, const wsp_token_data* tokens
 	uint32_t flags, wsp_segment* segs, int32_t cap, int32_t* n_segs )
 {
 	if( !m || !result || !n_segs || ( cap > 0 && !segs ) ) return fail( WSP_E_POINTER, "model/result/segs/n_segs" );
-	if( cap < 0 || result->n_tokens < 0 || result->n_tokens > result->n_sampled ) return fail( WSP_E_INVALIDARG, "cap/result" );
+	return windowSegments( [ m ]( int id ) { return wsp_model_token_text( m, id ); }, m->m->vocab.token_eot, m->m->vocab.token_beg, tokens, result,
+		seek, flags, segs, cap, n_segs );
+}
+wsp_status wsp_set_token_timestamps( wsp_context* c, int32_t on )
+{
+	if( !c ) return fail( WSP_E_POINTER, "context" );
+	return ctxSetTokenTimestamps( *c->c, on );
+}
+wsp_status wsp_window_token_times( wsp_context* c, int32_t chunk, const wsp_token_data* tokens, const wsp_window_result* result,
+	uint32_t flags, const wsp_token_time_params* p, wsp_segment* segs, int32_t cap, int32_t* n_segs, wsp_token_time* times )
+{
+	if( !c || !result || !p || !n_segs || ( cap > 0 && !segs ) ) return fail( WSP_E_POINTER, "context/result/params/segs/n_segs" );
 	const int len = result->failed ? 0 : result->n_tokens;
-	if( len > 0 && !tokens ) return fail( WSP_E_POINTER, "tokens" );
-	const int eot = m->m->vocab.token_eot, beg = m->m->vocab.token_beg;
-	const bool single = ( flags & WSP_SEGMENT_SINGLE ) != 0, special = ( flags & WSP_SEGMENT_PRINT_SPECIAL ) != 0;
-	const int64_t scale = ( flags & WSP_SEGMENT_SPEED_UP ) ? 2 : 1;
-	int n = 0;
-	auto emit = [ & ]( int64_t t0, int64_t t1, int i0, int i1 ) {
-		if( n < cap ) segs[ n ] = wsp_segment{ scale * t0, scale * t1, i0, i1 };
-		n++;
-	};
-	// whisper.cpp:3026-3119, with `text` reduced to whether it is empty: a segment's text is that of its tokens [i0, i1)
-	if( len > 0 )
-	{
-		int i0 = 0;
-		int64_t t0 = seek + 2 * ( (int64_t)tokens[ 0 ].tid - beg );
-		bool text = false;
+	if( result->n_tokens > 0 && ( !tokens || !times ) ) return fail( WSP_E_POINTER, "tokens/times" );
+	const Context& cx = *c->c;
+	if( cx.windowEnergyBatch < 1 ) return fail( WSP_E_INVALIDARG, "the last wsp_run_chunks_window call ran without token timestamps (or there was none)" );
+	if( chunk < 0 || chunk >= cx.windowEnergyBatch ) return fail( WSP_E_BOUNDS, "chunk outside the last window call's batch" );
+	return guarded( [ & ]() -> wsp_status {
+		const Engine& e = *cx.e;
+		auto textOf = [ & ]( int id ) -> const char* { return id >= 0 && id < (int)e.tokenText.size() ? e.tokenText[ (size_t)id ].c_str() : nullptr; };
+		std::vector<wsp_segment> cut( (size_t)len + 1 );
+		int32_t nCut = 0;
+		WSP_CHECK( windowSegments( textOf, e.tokEot, e.tokBeg, tokens, result, 0, flags, cut.data(), (int32_t)cut.size(), &nCut ) );
+		// whisper.cpp:3063-3070, 3107-3114: each segment's token times, then its wrapping, in order from the state of a new call
+		std::vector<wsp_token_time> tt( (size_t)len, wsp_token_time{ -1, -1, 0.0f } );
+		std::vector<float> vlen( (size_t)len );
+		std::vector<int> textLen( (size_t)len );
 		for( int i = 0; i < len; i++ )
 		{
-			const int id = tokens[ i ].id;
-			if( special || id < eot )
-			{
-				const char* t = wsp_model_token_text( m, id );
-				if( t && *t ) text = true;
-			}
-			if( id > beg && !single )
-			{
-				const int64_t t1 = seek + 2 * ( (int64_t)tokens[ i ].tid - beg );
-				if( text ) emit( t0, t1, i0, i + 1 );
-				text = false;
-				while( i < len && tokens[ i ].id > beg ) i++;
-				i--;
-				t0 = t1;
-				i0 = i + 1;
-			}
+			const char* t = textOf( tokens[ i ].id );
+			vlen[ (size_t)i ] = voiceLength( t );
+			textLen[ (size_t)i ] = t ? (int)strlen( t ) : 0;
 		}
-		if( text ) emit( t0, (int64_t)seek + result->seek_delta, i0, len );
-	}
-	*n_segs = n;
-	return n > cap ? fail( WSP_E_BOUNDS, "more segments than cap" ) : WSP_OK;
+		const float* energy = cx.energyHost + (size_t)chunk * cx.energyCap;
+		const int nSamples = cx.windowEnergyLen[ (size_t)chunk ];
+		TokenTimeState st;
+		std::vector<wsp_segment> out;
+		for( int k = 0; k < nCut; k++ )
+		{
+			const wsp_segment& g = cut[ (size_t)k ];
+			computeTokenTimes( tokens + g.i0, vlen.data() + g.i0, tt.data() + g.i0, g.i1 - g.i0, g.t0, g.t1, e.tokBeg, e.tokEot, energy, nSamples,
+				p->thold_pt, p->thold_ptsum, st );
+			if( p->max_len > 0 )
+			{
+				const size_t at = out.size();
+				out.resize( at + (size_t)( g.i1 - g.i0 ) + 1 );
+				const int pieces = wrapSegment( tokens, tt.data(), textLen.data(), g.i0, g.i1, g.t0, g.t1, e.tokEot, p->max_len, out.data() + at,
+					g.i1 - g.i0 + 1 );
+				out.resize( at + (size_t)pieces );
+			}
+			else out.push_back( g );
+		}
+		*n_segs = (int32_t)out.size();
+		if( (int32_t)out.size() > cap ) return fail( WSP_E_BOUNDS, "more segments than cap" );
+		std::copy( out.begin(), out.end(), segs );
+		for( int i = 0; i < result->n_tokens; i++ ) times[ i ] = i < len ? tt[ (size_t)i ] : wsp_token_time{ -1, -1, 0.0f };
+		return WSP_OK;
+	} );
 }
 
 wsp_status wsp_upload_pcm( wsp_context* c, int32_t slot, const float* pcm, int32_t n_samples )
@@ -421,6 +485,7 @@ wsp_status wsp_get_tensor( wsp_context* cc, const char* name, int32_t slot, floa
 		return WSP_OK;
 	}
 	else if( nm == "dec.x" ) { f32 = c.xd; n = (size_t)d * 8; }
+	else if( nm == "energy" ) { f32 = c.energy + (size_t)slot * c.energyCap; n = (size_t)c.energyLen[ (size_t)slot ]; }
 	else return fail( WSP_E_INVALIDARG, "unknown tensor name " + nm );
 	*n_floats = n;
 	if( !dst ) return WSP_OK;
@@ -688,6 +753,61 @@ wsp_status wsp_test_window_rule( const int32_t rule4[ 4 ], int32_t n_max, int32_
 	*n_steps = i < n ? i + 1 : n;
 	const int32_t o[ 5 ] = { s.hasTs, s.seekDelta, s.resultLen, s.failed, s.ended };
 	memcpy( out5, o, sizeof( o ) );
+	return WSP_OK;
+}
+
+wsp_status wsp_test_token_times( const wsp_token_data* tokens, const float* vlen, int32_t n, int64_t t0, int64_t t1, const int32_t special2[ 2 ],
+	const float* energy, int32_t n_samples, float thold_pt, float thold_ptsum, int64_t state3[ 3 ], wsp_token_time* times )
+{
+	if( !special2 || !state3 || ( n > 0 && ( !tokens || !vlen || !times ) ) || ( n_samples > 0 && !energy ) ) return fail( WSP_E_POINTER, "tokens/vlen/times/energy/state" );
+	if( n < 0 || n_samples < 0 ) return fail( WSP_E_INVALIDARG, "n / n_samples" );
+	TokenTimeState st{ state3[ 0 ], state3[ 1 ], (int)state3[ 2 ] };
+	if( !computeTokenTimes( tokens, vlen, times, n, t0, t1, special2[ 0 ], special2[ 1 ], energy, n_samples, thold_pt, thold_ptsum, st ) ) return WSP_S_FALSE;
+	state3[ 0 ] = st.tBeg; state3[ 1 ] = st.tLast; state3[ 2 ] = st.tidLast;
+	return WSP_OK;
+}
+
+wsp_status wsp_test_signal_energy( int32_t device, const float* const* pcm, const int32_t* n_samples, int32_t batch, float* const* energy,
+	int32_t iters, float* ms )
+{
+	if( !pcm || !n_samples || !energy ) return fail( WSP_E_POINTER, "pcm/n_samples/energy" );
+	if( batch < 1 || batch > kern::ENERGY_BATCH ) return fail( WSP_E_INVALIDARG, "batch" );
+	size_t most = 1;
+	for( int b = 0; b < batch; b++ )
+	{
+		if( n_samples[ b ] < 0 || ( n_samples[ b ] > 0 && ( !pcm[ b ] || !energy[ b ] ) ) ) return fail( WSP_E_INVALIDARG, "n_samples / pointers" );
+		most = std::max( most, (size_t)n_samples[ b ] );
+	}
+	WSP_CHECK( requireSm90( device ) );
+	DevTmp<float> dIn, dOut;
+	WSP_CUDA( dIn.alloc( (size_t)batch * most ) );
+	WSP_CUDA( dOut.alloc( (size_t)batch * most ) );
+	kern::EnergyBatch eb{};
+	eb.out = dOut.p; eb.stride = (int64_t)most; eb.count = batch;
+	for( int b = 0; b < batch; b++ )
+	{
+		eb.pcm[ b ] = dIn.p + (size_t)b * most;
+		eb.nSamples[ b ] = n_samples[ b ];
+		if( n_samples[ b ] ) WSP_CUDA( cudaMemcpy( dIn.p + (size_t)b * most, pcm[ b ], (size_t)n_samples[ b ] * 4, cudaMemcpyHostToDevice ) );
+	}
+	WSP_CUDA( kern::signalEnergy( eb, 0 ) );
+	WSP_CUDA( cudaDeviceSynchronize() );
+	if( iters > 0 )
+	{
+		cudaEvent_t e0, e1;
+		WSP_CUDA( cudaEventCreate( &e0 ) ); WSP_CUDA( cudaEventCreate( &e1 ) );
+		WSP_CUDA( cudaEventRecord( e0 ) );
+		for( int i = 0; i < iters; i++ ) WSP_CUDA( kern::signalEnergy( eb, 0 ) );
+		WSP_CUDA( cudaEventRecord( e1 ) );
+		WSP_CUDA( cudaDeviceSynchronize() );
+		float t = 0;
+		cudaEventElapsedTime( &t, e0, e1 );
+		if( ms ) *ms = t / iters;
+		cudaEventDestroy( e0 ); cudaEventDestroy( e1 );
+	}
+	g_launchCount.fetch_add( (uint64_t)( 1 + ( iters > 0 ? iters : 0 ) ) );
+	for( int b = 0; b < batch; b++ )
+		if( n_samples[ b ] ) WSP_CUDA( cudaMemcpy( energy[ b ], dOut.p + (size_t)b * most, (size_t)n_samples[ b ] * 4, cudaMemcpyDeviceToHost ) );
 	return WSP_OK;
 }
 

@@ -11,6 +11,7 @@
 #include "pcm_streamer.h"
 #include "capture_loop.h"
 #include "wav_reader.h"
+#include "token_times.h"
 #include "window_rule.h"
 #include <algorithm>
 #include <atomic>
@@ -446,12 +447,10 @@ namespace
 		std::vector<int32_t> promptPast;       // text context carried across windows and calls (whisper_context::prompt_past)
 		ResultData results;
 		mutable ResultObj* staticResult = nullptr;
-		// token-level timestamps (whisper_context::energy / t_beg / t_last / tid_last, whisper.cpp:425-431)
+		// token-level timestamps (whisper_context::energy / t_beg / t_last / tid_last, whisper.cpp:425-431); the energy is the device's
 		std::vector<float> energy;
-		int64_t tBeg = 0, tLast = 0;
-		int tidLast = 0;
-		void computeTokenTimestamps( size_t iSegment, float tholdPt, float tholdPtsum );
-		int wrapSegment( int maxLen );
+		wsp::TokenTimeState tokenTimeState;
+		int tokenTimesAndWrap( const sFullParams& params );
 		// what detectSpeaker looks at: the stereo samples of the clip being transcribed (ContextImpl::currentSpectrogram, ContextImpl.cpp:441-450)
 		bool insideRun = false;
 		const float* curStereo = nullptr;
@@ -715,207 +714,54 @@ namespace
 		return S_OK;
 	}
 
-	// ---- token-level timestamps and segment wrapping: restatement of the reference's "experimental" heuristics -------------------
-	// get_signal_energy (whisper.cpp:3356-3372): mean |x| over a window of 2 hw + 1 samples, f32 sums in the same order
-	static std::vector<float> signalEnergy( const float* signal, int nSamples, int hw )
+	// ---- token-level timestamps and segment wrapping (csrc/token_times.h) -------------------------------------------------------
+	// whisper_exp_compute_token_level_timestamps (whisper.cpp:3374-3600) over the last segment, then, with max_len, whisper_wrap_segment
+	// (:2713-2763) of it; returns the number of segments the last one became
+	int ContextObj::tokenTimesAndWrap( const sFullParams& params )
 	{
-		std::vector<float> result( (size_t)( nSamples > 0 ? nSamples : 0 ) );
-		for( int i = 0; i < nSamples; i++ )
+		ResultData::Seg& seg = results.segs.back();
+		const int n = (int)seg.tokens.size();
+		const int tokEot = eng->tokEot();
+		std::vector<wsp_token_data> td( (size_t)n );
+		std::vector<wsp_token_time> tt( (size_t)n );
+		std::vector<float> vlen( (size_t)n );
+		std::vector<int> textLen( (size_t)n );
+		for( int j = 0; j < n; j++ )
 		{
-			float sum = 0;
-			for( int j = -hw; j <= hw; j++ )
-				if( i + j >= 0 && i + j < nSamples ) sum += fabsf( signal[ i + j ] );
-			result[ (size_t)i ] = sum / ( 2 * hw + 1 );
+			const ResultData::Tok& tk = seg.tokens[ (size_t)j ];
+			const char* text = wsp_model_token_text( eng->model, tk.d.id );
+			td[ (size_t)j ] = tk.d;
+			tt[ (size_t)j ] = wsp_token_time{ tk.t0, tk.t1, tk.vlen };
+			vlen[ (size_t)j ] = wsp::voiceLength( text );
+			textLen[ (size_t)j ] = text ? (int)strlen( text ) : 0;
 		}
-		return result;
-	}
-	// voice_length (whisper.cpp:3330-3353): a cost that is high for text that takes longer to pronounce
-	static float voiceLength( const char* text )
-	{
-		float res = 0.0f;
-		for( const char* p = text ? text : ""; *p; p++ )
-		{
-			const char c = *p;
-			if( c == ' ' ) res += 0.01f;
-			else if( c == ',' ) res += 2.00f;
-			else if( c == '.' || c == '!' || c == '?' ) res += 3.00f;
-			else if( c >= '0' && c <= '9' ) res += 3.00f;
-			else res += 1.00f;
-		}
-		return res;
-	}
-	static int timestampToSample( int64_t t, int nSamples ) { return std::max( 0, std::min( nSamples - 1, (int)( ( t * 16000 ) / 100 ) ) ); }   // :3320-3322
-	static int64_t sampleToTimestamp( int iSample ) { return ( 100 * (int64_t)iSample ) / 16000; }                                            // :3324-3326
-
-	// whisper_exp_compute_token_level_timestamps (whisper.cpp:3374-3600), step by step: timestamps from confident timestamp tokens,
-	// the gaps split in proportion to the voice lengths, then every token grown / shrunk against the signal energy
-	void ContextObj::computeTokenTimestamps( size_t iSegment, float tholdPt, float tholdPtsum )
-	{
-		ResultData::Seg& segment = results.segs[ iSegment ];
-		auto& tokens = segment.tokens;
-		const int nSamples = (int)energy.size();
-		if( nSamples == 0 )
-		{
-			logMessage( eLogLevel::Warning, "computeTokenTimestamps: no signal data available" );
-			return;
-		}
-		const int64_t t0 = segment.t0, t1 = segment.t1;
-		const int n = (int)tokens.size();
-		if( n == 0 ) return;
-		if( n == 1 ) { tokens[ 0 ].t0 = t0; tokens[ 0 ].t1 = t1; return; }
-		const int tokBeg = eng->tokBeg(), tokEot = eng->tokEot();
-		for( int j = 0; j < n; ++j )
-		{
-			const wsp_token_data& token = tokens[ j ].d;
-			if( j == 0 )
-			{
-				if( token.id == tokBeg )
-				{
-					tokens[ j ].t0 = t0;
-					tokens[ j ].t1 = t0;
-					tokens[ j + 1 ].t0 = t0;
-					tBeg = t0; tLast = t0; tidLast = tokBeg;
-				}
-				else tokens[ j ].t0 = tLast;
-			}
-			const int64_t tt = tBeg + 2 * ( (int64_t)token.tid - tokBeg );
-			tokens[ j ].vlen = voiceLength( wsp_model_token_text( eng->model, token.id ) );
-			if( token.pt > tholdPt && token.ptsum > tholdPtsum && token.tid > tidLast && tt <= t1 )
-			{
-				if( j > 0 ) tokens[ j - 1 ].t1 = tt;
-				tokens[ j ].t0 = tt;
-				tidLast = token.tid;
-			}
-		}
-		tokens[ n - 2 ].t1 = t1;
-		tokens[ n - 1 ].t0 = t1;
-		tokens[ n - 1 ].t1 = t1;
-		tLast = t1;
-		// intervals of tokens with unknown timestamps: split proportionally to the voice lengths
-		{
-			int p0 = 0, p1 = 0;
-			while( true )
-			{
-				while( p1 < n && tokens[ p1 ].t1 < 0 ) p1++;
-				if( p1 >= n ) p1--;
-				if( p1 > p0 )
-				{
-					double psum = 0.0;
-					for( int j = p0; j <= p1; j++ ) psum += tokens[ j ].vlen;
-					const double dt = (double)( tokens[ p1 ].t1 - tokens[ p0 ].t0 );
-					for( int j = p0 + 1; j <= p1; j++ )
-					{
-						const double ct = tokens[ j - 1 ].t0 + dt * tokens[ j - 1 ].vlen / psum;
-						tokens[ j - 1 ].t1 = (int64_t)ct;
-						tokens[ j ].t0 = (int64_t)ct;
-					}
-				}
-				p1++;
-				p0 = p1;
-				if( p1 >= n ) break;
-			}
-		}
-		// fix up (just in case)
-		for( int j = 0; j < n - 1; j++ )
-		{
-			if( tokens[ j ].t1 < 0 ) tokens[ j + 1 ].t0 = tokens[ j ].t1;
-			if( j > 0 && tokens[ j - 1 ].t1 > tokens[ j ].t0 )
-			{
-				tokens[ j ].t0 = tokens[ j - 1 ].t1;
-				tokens[ j ].t1 = std::max( tokens[ j ].t0, tokens[ j ].t1 );
-			}
-		}
-		// VAD: expand or contract tokens based on voice activity
-		{
-			const int hw = 16000 / 8;
+		if( wsp::computeTokenTimes( td.data(), vlen.data(), tt.data(), n, seg.t0, seg.t1, eng->tokBeg(), tokEot, energy.data(), (int)energy.size(),
+				params.thold_pt, params.thold_ptsum, tokenTimeState ) )
 			for( int j = 0; j < n; j++ )
 			{
-				if( tokens[ j ].d.id >= tokEot ) continue;
-				int s0 = timestampToSample( tokens[ j ].t0, nSamples );
-				int s1 = timestampToSample( tokens[ j ].t1, nSamples );
-				const int ss0 = std::max( s0 - hw, 0 );
-				const int ss1 = std::min( s1 + hw, nSamples );
-				const int ns = ss1 - ss0;
-				float sum = 0.0f;
-				for( int k = ss0; k < ss1; k++ ) sum += energy[ (size_t)k ];
-				const float thold = (float)( 0.5 * sum / ns );
-				{
-					int k = s0;
-					if( energy[ (size_t)k ] > thold && j > 0 )
-					{
-						while( k > 0 && energy[ (size_t)k ] > thold ) k--;
-						tokens[ j ].t0 = sampleToTimestamp( k );
-						if( tokens[ j ].t0 < tokens[ j - 1 ].t1 ) tokens[ j ].t0 = tokens[ j - 1 ].t1;
-						else s0 = k;
-					}
-					else
-					{
-						while( energy[ (size_t)k ] < thold && k < s1 ) k++;
-						s0 = k;
-						tokens[ j ].t0 = sampleToTimestamp( k );
-					}
-				}
-				{
-					int k = s1;
-					if( energy[ (size_t)k ] > thold )
-					{
-						while( k < nSamples - 1 && energy[ (size_t)k ] > thold ) k++;
-						tokens[ j ].t1 = sampleToTimestamp( k );
-						// (the reference tests `j < ns - 1` and then reads tokens[j + 1]: past the end for the last token of a segment
-						// that does not close with a timestamp — undefined there, skipped here)
-						if( j < ns - 1 && j + 1 < n && tokens[ j ].t1 > tokens[ j + 1 ].t0 ) tokens[ j ].t1 = tokens[ j + 1 ].t0;
-						else s1 = k;
-					}
-					else
-					{
-						while( energy[ (size_t)k ] < thold && k > s0 ) k--;
-						s1 = k;
-						tokens[ j ].t1 = sampleToTimestamp( k );
-					}
-				}
+				ResultData::Tok& tk = seg.tokens[ (size_t)j ];
+				tk.t0 = tt[ (size_t)j ].t0; tk.t1 = tt[ (size_t)j ].t1; tk.vlen = tt[ (size_t)j ].vlen;
 			}
-		}
-	}
-
-	// whisper_wrap_segment (whisper.cpp:2713-2763): wrap the last segment to max_len characters; returns the number of new segments
-	int ContextObj::wrapSegment( int maxLen )
-	{
-		ResultData::Seg segment = results.segs.back();
-		int res = 1, acc = 0;
-		std::string text;
-		const int tokEot = eng->tokEot();
-		for( int i = 0; i < (int)segment.tokens.size(); i++ )
+		else logMessage( eLogLevel::Warning, "computeTokenTimestamps: no signal data available" );
+		if( params.max_len <= 0 ) return 1;
+		std::vector<wsp_segment> pieces( (size_t)n + 1 );
+		const int nNew = wsp::wrapSegment( td.data(), tt.data(), textLen.data(), 0, n, seg.t0, seg.t1, tokEot, params.max_len, pieces.data(), n + 1 );
+		ResultData::Seg whole = std::move( seg );
+		results.segs.pop_back();
+		for( int k = 0; k < nNew; k++ )
 		{
-			const ResultData::Tok& token = segment.tokens[ (size_t)i ];
-			if( token.d.id >= tokEot ) continue;
-			const char* txt = wsp_model_token_text( eng->model, token.d.id );
-			if( !txt ) txt = "";
-			const int cur = (int)strlen( txt );
-			if( acc + cur > maxLen && i > 0 )
+			const wsp_segment& pc = pieces[ (size_t)k ];
+			ResultData::Seg s;
+			s.t0 = pc.t0; s.t1 = pc.t1;
+			s.tokens.assign( whole.tokens.begin() + pc.i0, whole.tokens.begin() + pc.i1 );
+			for( const auto& tk : s.tokens )                   // a wrapped segment's text is that of its non-special tokens (:2724-2727)
 			{
-				// split here
-				results.segs.back().text = std::move( text );
-				results.segs.back().t1 = token.t0;
-				results.segs.back().tokens.resize( (size_t)i );
-				ResultData::Seg next;
-				next.t0 = token.t0;
-				next.t1 = segment.t1;
-				next.tokens.assign( segment.tokens.begin() + i, segment.tokens.end() );
-				results.segs.push_back( std::move( next ) );
-				acc = 0;
-				text.clear();
-				segment = results.segs.back();
-				i = -1;
-				res++;
+				const char* text = tk.d.id < tokEot ? wsp_model_token_text( eng->model, tk.d.id ) : nullptr;
+				if( text ) s.text += text;
 			}
-			else
-			{
-				acc += cur;
-				text += txt;
-			}
+			results.segs.push_back( std::move( s ) );
 		}
-		results.segs.back().text = std::move( text );
-		return res;
+		return nNew;
 	}
 
 	// whisper_lang_auto_detect (whisper.cpp:2428-2495): encode at offset 0, decode [sot], most probable language token
@@ -958,12 +804,17 @@ namespace
 		const float* pcm = buffer->getPcmMono();
 		const int nSamples = (int)buffer->countSamples();
 		if( !pcm && nSamples > 0 ) return E_POINTER;
-		HR( check( wsp_pcm_to_mel( ctx, 0, pcm, nSamples ), "wsp_pcm_to_mel" ) );                 // :2782
+		// with token timestamps the clip's signal energy (get_signal_energy, :2803-2808) is computed on the device with its log-mel
 		const bool tokenTimestamps = params.flag( eFullParamsFlags::TokenTimestamps );
+		HR( check( wsp_set_token_timestamps( ctx, tokenTimestamps ? 1 : 0 ), "wsp_set_token_timestamps" ) );
+		HR( check( wsp_pcm_to_mel( ctx, 0, pcm, nSamples ), "wsp_pcm_to_mel" ) );                 // :2782
 		if( tokenTimestamps )                                                                      // :2803-2808
 		{
-			tBeg = 0; tLast = 0; tidLast = 0;
-			energy = signalEnergy( pcm, nSamples, 32 );
+			tokenTimeState = wsp::TokenTimeState();
+			size_t n = 0;
+			HR( check( wsp_get_tensor( ctx, "energy", 0, nullptr, 0, &n ), "wsp_get_tensor" ) );
+			energy.resize( n );
+			if( n ) HR( check( wsp_get_tensor( ctx, "energy", 0, energy.data(), n, &n ), "wsp_get_tensor" ) );
 		}
 		MelSource mel;
 		mel.nLen = wsp_mel_len( ctx, 0 );
@@ -1222,8 +1073,7 @@ namespace
 				int nNew = 1;
 				if( tokenTimestamps )                                                              // :3063-3070, 3107-3114
 				{
-					computeTokenTimestamps( results.segs.size() - 1, params.thold_pt, params.thold_ptsum );
-					if( params.max_len > 0 ) nNew = wrapSegment( params.max_len );
+					nNew = tokenTimesAndWrap( params );
 				}
 				if( params.new_segment_callback )
 				{

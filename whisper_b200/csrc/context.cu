@@ -2,9 +2,11 @@
 // Reference: WhisperContext::encode / ::decode (Whisper/Whisper/WhisperContext.cpp:310-388, 578-639); oracle whisper_encode /
 // whisper_decode (Whisper/source/whisper.cpp:1084-1872).  All launches go to one stream; the N = 1 decoder step is a CUDA graph.
 #include "engine.h"
+#include <algorithm>
 #include <math.h>
 #include <memory>
 #include <stdlib.h>
+#include <string.h>
 
 namespace wsp
 {
@@ -37,9 +39,10 @@ namespace wsp
 		for( auto& v : prof.pool ) cudaEventDestroy( v );
 		for( auto& v : timerEv ) if( v ) cudaEventDestroy( v );
 		void* bufs[] = { stepLayers, flowBias, flowExch, flowCtrl, megaBarrier, stepMarks, melMax, pcmDev, melF16, conv1, x, xn, q, k, vt, attn, h, crossK, crossV, selfK, selfV, xd, qd, attnD, hD, logits, probs, tieScratch,
-			tokensDev, dNPast, sampled, history, endStep, langIds, langProbs, winCtl, winState, tokenLog };
+			tokensDev, dNPast, sampled, history, endStep, langIds, langProbs, winCtl, winState, tokenLog, energy };
 		for( void* b : bufs ) if( b ) cudaFree( b );
 		if( nEndedHost ) cudaFreeHost( nEndedHost );
+		if( energyHost ) cudaFreeHost( energyHost );
 		for( auto& v : ev ) if( v ) cudaEventDestroy( v );
 		for( auto& v : blockEv ) if( v ) cudaEventDestroy( v );
 		if( stream ) cudaStreamDestroy( stream );
@@ -65,6 +68,7 @@ namespace wsp
 		for( auto& v : c.timerEv ) WSP_CUDA( cudaEventCreate( &v ) );
 		for( auto& v : c.blockEv ) WSP_CUDA( cudaEventCreateWithFlags( &v, cudaEventDisableTiming ) );
 		c.slots.resize( maxBatch );
+		c.energyLen.assign( maxBatch, 0 );
 		const size_t B = (size_t)maxBatch;
 		WSP_CHECK( devAlloc( c.melMax, B ) );
 		// the halo rows are rewritten by every encode (mel_window_kernel, EPI_CONV1) except row 0, which no packing moves
@@ -267,6 +271,64 @@ namespace wsp
 		return WSP_OK;
 	}
 
+	// room for `samples` of signal energy per slot, on the device and, for window calls, in pinned host memory; what the slots hold
+	// is kept
+	static int ensureEnergy( Context& c, size_t samples, bool host )
+	{
+		if( samples > c.energyCap )
+		{
+			WSP_CUDA( cudaStreamSynchronize( c.stream ) );
+			float* grown = nullptr;
+			WSP_CHECK( devAlloc( grown, (size_t)c.maxB * samples ) );
+			if( c.energy )
+			{
+				WSP_CUDA( cudaMemcpy2D( grown, samples * 4, c.energy, c.energyCap * 4, c.energyCap * 4, (size_t)c.maxB, cudaMemcpyDeviceToDevice ) );
+				cudaFree( c.energy );
+			}
+			if( c.energyHost )
+			{
+				float* grownHost = nullptr;
+				WSP_CUDA( cudaHostAlloc( (void**)&grownHost, (size_t)c.maxB * samples * 4, cudaHostAllocDefault ) );
+				for( size_t b = 0; b < (size_t)c.maxB; b++ ) memcpy( grownHost + b * samples, c.energyHost + b * c.energyCap, c.energyCap * 4 );
+				cudaFreeHost( c.energyHost );
+				c.energyHost = grownHost;
+			}
+			c.devBytes += (uint64_t)c.maxB * ( samples - c.energyCap ) * 4;
+			c.energy = grown;
+			c.energyCap = samples;
+		}
+		if( host && !c.energyHost ) WSP_CUDA( cudaHostAlloc( (void**)&c.energyHost, (size_t)c.maxB * c.energyCap * 4, cudaHostAllocDefault ) );
+		return WSP_OK;
+	}
+	// signal energy of chunks [0, batch) into slots [slot0, slot0 + batch) in one launch; pcmOf( b ) / samplesOf( b ) name chunk b's
+	// device PCM.  ensureEnergy has made room.
+	template<class P, class N>
+	static int energyFromDevicePcm( Context& c, int slot0, int batch, P pcmOf, N samplesOf )
+	{
+		kern::EnergyBatch eb{};
+		eb.out = c.energy + (size_t)slot0 * c.energyCap;
+		eb.stride = (int64_t)c.energyCap;
+		eb.count = batch;
+		for( int b = 0; b < batch; b++ )
+		{
+			eb.pcm[ b ] = pcmOf( b );
+			eb.nSamples[ b ] = samplesOf( b );
+			c.energyLen[ (size_t)( slot0 + b ) ] = eb.nSamples[ b ];
+		}
+		WSP_CUDA( kern::signalEnergy( eb, c.stream ) );
+		launched();
+		return WSP_OK;
+	}
+	static_assert( kern::ENERGY_BATCH >= 256, "one energy launch covers the largest context" );
+
+	// whisper_full_params::token_timestamps: the signal energy of window calls and pcm_to_mel
+	int ctxSetTokenTimestamps( Context& c, int on )
+	{
+		if( on != 0 && on != 1 ) return fail( WSP_E_INVALIDARG, "token timestamps must be 0 or 1" );
+		c.tokenTimestamps = on != 0;
+		return WSP_OK;
+	}
+
 	// one clip's host PCM into c.pcmDev, then melOf() enqueues its log-mel; both are timed as the mel stage
 	template<class M>
 	static int pcmToMelTimed( Context& c, const float* pcmHost, int nSamples, M melOf )
@@ -283,8 +345,12 @@ namespace wsp
 	int ctxPcmToMel( Context& c, int slot, const float* pcmHost, int nSamples )
 	{
 		if( ( !pcmHost && nSamples != 0 ) || nSamples < 0 ) return fail( WSP_E_INVALIDARG, "pcm" );
+		if( c.tokenTimestamps ) WSP_CHECK( ensureEnergy( c, (size_t)( nSamples > 0 ? nSamples : 1 ), false ) );
 		return pcmToMelTimed( c, pcmHost, nSamples, [ & ]() -> int {
-			return melBatchFromDevicePcm( c, slot, 1, [ & ]( int ) { return (const float*)c.pcmDev; }, [ & ]( int ) { return nSamples; } );
+			auto pcmOf = [ & ]( int ) { return (const float*)c.pcmDev; };
+			auto samplesOf = [ & ]( int ) { return nSamples; };
+			WSP_CHECK( melBatchFromDevicePcm( c, slot, 1, pcmOf, samplesOf ) );
+			return c.tokenTimestamps ? energyFromDevicePcm( c, slot, 1, pcmOf, samplesOf ) : WSP_OK;
 		} );
 	}
 
@@ -778,12 +844,29 @@ namespace wsp
 		c.lastLangIds.clear();
 		c.lastLangProbs.clear();
 		WSP_CUDA( cudaSetDevice( c.e->device ) );
+		// a window call with token timestamps on computes every chunk's signal energy right after the log-mel
+		const bool energy = window && c.tokenTimestamps;
+		if( window ) c.windowEnergyBatch = 0;
+		std::vector<int> energyLen( energy ? (size_t)batch : 0 );
+		if( energy )
+		{
+			size_t most = 1;
+			for( int b = 0; b < batch; b++ )
+			{
+				energyLen[ (size_t)b ] = resident ? c.slots[ b ].pcmSamples : nSamples[ b ];
+				most = std::max( most, (size_t)energyLen[ (size_t)b ] );
+			}
+			WSP_CHECK( ensureEnergy( c, most, true ) );
+		}
 		cudaStream_t s = c.stream;
 		WSP_CUDA( cudaEventRecord( c.ev[ 0 ], s ) );
 		if( resident )
 		{
 			// inputs already in HBM (wsp_upload_pcm): the log-mel front end still runs inside the timed region
-			WSP_CHECK( melBatchFromDevicePcm( c, 0, batch, [ & ]( int b ) { return (const float*)c.slots[ b ].pcm; }, [ & ]( int b ) { return c.slots[ b ].pcmSamples; } ) );
+			auto pcmOf = [ & ]( int b ) { return (const float*)c.slots[ b ].pcm; };
+			auto samplesOf = [ & ]( int b ) { return c.slots[ b ].pcmSamples; };
+			WSP_CHECK( melBatchFromDevicePcm( c, 0, batch, pcmOf, samplesOf ) );
+			if( energy ) WSP_CHECK( energyFromDevicePcm( c, 0, batch, pcmOf, samplesOf ) );
 		}
 		else
 		{
@@ -799,7 +882,10 @@ namespace wsp
 				offs[ (size_t)b ] = off;
 				off += (size_t)nSamples[ b ];
 			}
-			WSP_CHECK( melBatchFromDevicePcm( c, 0, batch, [ & ]( int b ) { return (const float*)( c.pcmDev + offs[ (size_t)b ] ); }, [ & ]( int b ) { return (int)nSamples[ b ]; } ) );
+			auto pcmOf = [ & ]( int b ) { return (const float*)( c.pcmDev + offs[ (size_t)b ] ); };
+			auto samplesOf = [ & ]( int b ) { return (int)nSamples[ b ]; };
+			WSP_CHECK( melBatchFromDevicePcm( c, 0, batch, pcmOf, samplesOf ) );
+			if( energy ) WSP_CHECK( energyFromDevicePcm( c, 0, batch, pcmOf, samplesOf ) );
 		}
 		WSP_CUDA( cudaEventRecord( c.ev[ 1 ], s ) );
 		WSP_CHECK( encodeAsync( c, nullptr, batch ) );
@@ -884,6 +970,9 @@ namespace wsp
 			WSP_CUDA( cudaMemcpyAsync( winSt.data(), c.winState, winSt.size() * sizeof( wsp::WindowState ), cudaMemcpyDeviceToHost, s ) );
 			WSP_CUDA( cudaMemcpyAsync( tdLog.data(), c.tokenLog, tdLog.size() * sizeof( kern::TokenData ), cudaMemcpyDeviceToHost, s ) );
 		}
+		for( size_t b = 0; b < energyLen.size(); b++ )
+			if( energyLen[ b ] > 0 )
+				WSP_CUDA( cudaMemcpyAsync( c.energyHost + b * c.energyCap, c.energy + b * c.energyCap, (size_t)energyLen[ b ] * 4, cudaMemcpyDeviceToHost, s ) );
 		std::vector<int32_t> langIds( detect ? (size_t)batch : 0 );
 		std::vector<float> langProbs( detect ? (size_t)batch * c.e->nLangs : 0 );
 		if( detect )
@@ -894,6 +983,11 @@ namespace wsp
 		WSP_CUDA( cudaStreamSynchronize( s ) );
 		c.lastLangIds.swap( langIds );
 		c.lastLangProbs.swap( langProbs );
+		if( energy )
+		{
+			c.windowEnergyBatch = batch;
+			c.windowEnergyLen.swap( energyLen );
+		}
 		if( window )
 			for( int b = 0; b < batch; b++ )
 			{

@@ -164,6 +164,7 @@ namespace wsp
 		e->tokSolm = m.vocab.token_solm; e->tokNot = m.vocab.token_not; e->tokBeg = m.vocab.token_beg;
 		// the reference's g_lang: language l is token sot + 1 + l, up to the task tokens (whisper.cpp:2466-2468)
 		e->nLangs = m.vocab.multilingual() ? Vocab::token_translate - m.vocab.token_sot - 1 : 0;
+		e->tokenText = m.vocab.id_to_token;
 		const HParams& h = m.hp;
 		const int d = h.n_audio_state;
 		const size_t dd = (size_t)d * d;

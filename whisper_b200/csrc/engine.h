@@ -82,6 +82,7 @@ namespace wsp
 		std::vector<DecLayerW> dec;
 		kern::MelTables mel;
 		kern::MelTables melVocoder;   // the phase vocoder's 800-point window and twiddles, mel's filters (speed-up)
+		std::vector<std::string> tokenText;   // the vocabulary, for the host-side segment rules of wsp_window_token_times
 
 		~Engine();
 	};
@@ -183,6 +184,14 @@ namespace wsp
 		float* langProbs = nullptr;     // [maxB][nLangs]
 		std::vector<int32_t> lastLangIds;   // host copies from the last run_chunks* call (wsp_get_chunk_languages); empty: it had no sentinel
 		std::vector<float> lastLangProbs;   // [batch][nLangs]
+		// signal energy of token-level timestamps (wsp_set_token_timestamps): computed only while tokenTimestamps is set
+		bool tokenTimestamps = false;
+		float* energy = nullptr;        // [maxB][energyCap] on the device
+		float* energyHost = nullptr;    // [maxB][energyCap] pinned: the last window call's energy, copied back with its tokens
+		size_t energyCap = 0;
+		std::vector<int> energyLen;     // [maxB] samples of each slot's device energy
+		int windowEnergyBatch = 0;      // batch of the last wsp_run_chunks_window call if it computed the energy, else 0
+		std::vector<int> windowEnergyLen;   // [that batch] samples of each chunk's energy in energyHost
 		int lastLogitRows = 0;
 		int nPastHost = 0;              // host mirror of the device-resident n_past (it advances on the device between graph replays)
 		int debugEncLayers = -1;
@@ -234,6 +243,7 @@ namespace wsp
 	int ctxEncode( Context& c, const int32_t* offsets, int batch );
 	int ctxSetAudioCtx( Context& c, int n );
 	int ctxSetSpeedUp( Context& c, int on );
+	int ctxSetTokenTimestamps( Context& c, int on );
 	int ctxDecode( Context& c, const int32_t* tokensHost, int nTokens, int nPast, int batch, uint32_t flags, wsp_token_data* sampledHost );
 	int ctxUploadPcm( Context& c, int slot, const float* pcmHost, int nSamples );
 	int ctxProfileDecode( Context& c, int batch, int nSteps, float* msByKind, int* launchesByKind );

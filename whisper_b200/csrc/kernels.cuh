@@ -59,6 +59,21 @@ namespace kern
 	// frames = 2 * audio_ctx (3000 by default)
 	cudaError_t melWindow( const float* mel, int nLen, int offset, __half* dst, int frames, cudaStream_t s );
 
+	// ---- signal energy of token-level timestamps (get_signal_energy, whisper.cpp:3356-3372) ----------------------------------
+	// every chunk of a batch in one launch: chunk b's pcm[b][nSamples[b]] -> out[b * stride + i] = (sum over j = -32..32 with
+	// 0 <= i + j < n of |x[i + j]|) / 65, the sum in f32 in that order of j, so the result is bit-identical to the reference's
+	constexpr int ENERGY_BATCH = 256;
+	constexpr int ENERGY_HW = 32;
+	struct EnergyBatch
+	{
+		const float* pcm[ ENERGY_BATCH ];
+		int nSamples[ ENERGY_BATCH ];
+		float* out;                    // [count][stride]
+		int64_t stride;
+		int count;
+	};
+	cudaError_t signalEnergy( const EnergyBatch& eb, cudaStream_t s );
+
 	// ---- LayerNorm + affine -> f16 (a5, a11) -------------------------------------------------------------------------
 	cudaError_t layerNormF16( const float* x, const float* gamma, const float* beta, __half* out, int rows, int d, cudaStream_t s );
 

@@ -221,6 +221,45 @@ namespace kern
 	}
 
 	// ---------------------------------------------------------------------------------------------------------------
+	// signal energy (get_signal_energy, whisper.cpp:3356-3372): one CTA per ENERGY_TILE samples of one chunk (blockIdx.y).  The CTA
+	// stages |x| of its tile and the 32-sample halo on each side in shared memory, zero outside the clip, and each thread adds its
+	// sample's 65 terms in the reference's order: a +0.0f in place of a skipped term leaves an f32 sum unchanged, so the result is the
+	// reference's bit for bit.  The division is IEEE (no fast math in this build).
+	constexpr int ENERGY_TILE = 512;
+	static_assert( sizeof( EnergyBatch ) <= 4096, "EnergyBatch is passed by value as a kernel parameter" );
+	__global__ void __launch_bounds__( ENERGY_TILE )
+		signal_energy_kernel( const EnergyBatch eb )
+	{
+		__shared__ float sx[ ENERGY_TILE + 2 * ENERGY_HW ];
+		const int b = blockIdx.y;
+		const int n = eb.nSamples[ b ];
+		const int i0 = blockIdx.x * ENERGY_TILE;
+		if( i0 >= n ) return;
+		const float* __restrict__ x = eb.pcm[ b ];
+		for( int k = threadIdx.x; k < ENERGY_TILE + 2 * ENERGY_HW; k += ENERGY_TILE )
+		{
+			const int idx = i0 - ENERGY_HW + k;
+			sx[ k ] = idx >= 0 && idx < n ? fabsf( x[ idx ] ) : 0.0f;
+		}
+		__syncthreads();
+		const int i = i0 + threadIdx.x;
+		if( i >= n ) return;
+		float sum = 0.0f;
+#pragma unroll
+		for( int j = 0; j <= 2 * ENERGY_HW; j++ ) sum += sx[ threadIdx.x + j ];
+		eb.out[ b * eb.stride + i ] = sum / (float)( 2 * ENERGY_HW + 1 );
+	}
+	cudaError_t signalEnergy( const EnergyBatch& eb, cudaStream_t s )
+	{
+		if( eb.count < 1 || eb.count > ENERGY_BATCH ) return cudaErrorInvalidValue;
+		int maxN = 0;
+		for( int b = 0; b < eb.count; b++ ) maxN = eb.nSamples[ b ] > maxN ? eb.nSamples[ b ] : maxN;
+		const int tiles = ( maxN + ENERGY_TILE - 1 ) / ENERGY_TILE;   // one launch even for a batch of empty clips
+		signal_energy_kernel<<<dim3( tiles > 0 ? tiles : 1, eb.count ), ENERGY_TILE, 0, s>>>( eb );
+		return cudaGetLastError();
+	}
+
+	// ---------------------------------------------------------------------------------------------------------------
 	// LayerNorm (eps 1e-5 inside the sqrt) + affine -> f16: one warp per row, the row stays in registers.
 	// Oracle: ggml_compute_forward_norm_f32 (ggml.c:4098-4156) then mul/add with gamma/beta (whisper.cpp:1190-1198);
 	// the f16 rounding is the activation conversion the next mul_mat performs (ggml.c:4592-4603).
