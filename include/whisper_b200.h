@@ -25,6 +25,8 @@
  *   wsp_set_token_timestamps  whisper_full_params::token_timestamps (Whisper/API/sFullParams.h eFullParamsFlags::TokenTimestamps): the
  *                             signal energy of get_signal_energy (whisper.cpp:3356-3372), computed on the device
  *   wsp_window_token_times    those segments with whisper_full's token times (whisper.cpp:3374-3600) and max_len wrapping (:2713-2763)
+ *   wsp_upload_pcm_stereo     a stereo chunk, downmixed on the device as Whisper/MF/AudioBuffer.cpp:57-93 (appendDownmixedStereo)
+ *   wsp_chunk_speakers        iContext::detectSpeaker (Whisper/Whisper/ContextImpl.diarize.cpp:73-108) for every segment of a batch
  *   wsp_get_tensor            the reference's named trace points, Whisper/Utils/Trace/tracing.h (names as in whisper.cpp:1121-1869)
  *
  * Error handling mirrors the reference's HRESULT convention (SURVEY.md §8b): every function returns a wsp_status that the COM
@@ -282,6 +284,43 @@ typedef struct wsp_token_time_params
 wsp_status wsp_window_token_times( wsp_context* c, int32_t chunk, const wsp_token_data* tokens, const wsp_window_result* result,
 	uint32_t flags, const wsp_token_time_params* p, wsp_segment* segs, int32_t cap, int32_t* n_segs, wsp_token_time* times );
 
+/* ---- stereo chunks and per-segment speakers on the batch path (iContext::detectSpeaker, the CLI's --diarize) ---- */
+/* Interleaved 16 kHz f32 stereo lr[n_frames][2] (left, right) into slot `slot`: the pairs are kept on the device, and one kernel launch
+ * writes the slot's resident mono PCM as (l + r) * 0.5f per frame, AudioBuffer::appendDownmixedStereo's mix (Whisper/MF/AudioBuffer.cpp:
+ * 57-93) and the one the WAV reader gives runFull for two channels, bit for bit.  wsp_run_chunks_resident, and wsp_run_chunks_until_eot /
+ * wsp_run_chunks_window with pcm == NULL, then run from that mono exactly as after wsp_upload_pcm of it (language sentinel, audio_ctx,
+ * speed-up and token timestamps included).  Returns once the slot holds the data.  The pairs stay the slot's stereo until the next
+ * wsp_upload_pcm_stereo or wsp_upload_pcm to the slot: wsp_upload_pcm drops them.  Their device memory counts in
+ * wsp_context_device_bytes.  lr may be NULL when n_frames is 0; a slot outside max_batch is WSP_E_BOUNDS, a negative n_frames
+ * WSP_E_INVALIDARG. */
+wsp_status wsp_upload_pcm_stereo( wsp_context* c, int32_t slot, const float* lr, int32_t n_frames );
+/* iContext::detectSpeaker's answers (Whisper/Whisper/ContextImpl.diarize.cpp:73-108), the values of eSpeakerChannel */
+enum
+{
+	WSP_SPEAKER_UNSURE = 0,
+	WSP_SPEAKER_LEFT = 1,
+	WSP_SPEAKER_RIGHT = 2,
+	WSP_SPEAKER_NO_STEREO = 255,
+	WSP_SPEAKER_OUT_OF_RANGE = -1,   /* the segment starts outside the clip: the reference's E_BOUNDS (Spectrogram.cpp:142-168) */
+};
+/* The speaker of every segment of a batch, as detectSpeaker answers it for the clip alone, bit for bit, in one kernel launch with one
+ * copy in and one copy out.  Chunk b's segments are segs[seg_start[b] .. seg_start[b + 1]) and are read against slot b's stereo;
+ * speakers[i] receives segment i's answer.  The segments are whatever the caller emits for the chunk, wsp_window_segments or the wrapped
+ * segments of wsp_window_token_times: t0 / t1 in 10 ms units from the chunk's start (under speed-up already doubled, so real time over
+ * the original samples).  For a segment with begin = t0, end = t1:
+ *   end - begin <= 0                                   WSP_SPEAKER_UNSURE
+ *   else, slot b holds no stereo (or none of n_frames)  WSP_SPEAKER_NO_STEREO
+ *   else, begin < 0 or begin * 160 >= n_frames          WSP_SPEAKER_OUT_OF_RANGE
+ *   else the frames [begin * 160, end * 160) cut at the end of the clip (the reference's zero fill after it adds nothing): |L| and |R|
+ *   are summed in the reference's SSE lane order, even frames and odd frames in separate f32 accumulators, each a chain in frame order,
+ *   then left = L even + L odd and right = R even + R odd (ContextImpl.diarize.cpp:17-52), and the answer is
+ *   (left > right * 1.1f) | (right > left * 1.1f) << 1 (:54-70): WSP_SPEAKER_LEFT, WSP_SPEAKER_RIGHT or WSP_SPEAKER_UNSURE.
+ * The chains are kept as chains on the device: a pairwise sum would round differently and move decisions within rounding of 1.1.
+ * Every argument is checked before anything is enqueued: a null pointer is WSP_E_POINTER (segs may be NULL when seg_start[batch] is 0),
+ * seg_start[0] != 0 or a decreasing seg_start is WSP_E_INVALIDARG, a batch outside [1, max_batch] is WSP_E_BOUNDS.  A batch without
+ * segments launches nothing. */
+wsp_status wsp_chunk_speakers( wsp_context* c, int32_t batch, const int32_t* seg_start, const wsp_segment* segs, int32_t* speakers );
+
 /* ---- several devices in one process (csrc/replicas.cpp) ----
  * Chunks are independent (SURVEY.md §8e): one engine + context per listed device (a device may be listed twice: two contexts on one
  * GPU), the model file read ONCE and its image copied device-to-device from devices[0] (cudaMemcpyPeer over NVLink) — the C++ form of
@@ -328,7 +367,9 @@ wsp_status wsp_profile_decode( wsp_context* c, int32_t batch, int32_t n_steps, f
  *   "cross_k", "cross_v"   [L][H][n][64] f16 cross-attention memories (K scaled by 64^-0.25)
  *   "self_k", "self_v"     [L][H][n_text_ctx][64] f16 decoder self-KV cache (K scaled by 64^-0.25); row j = text position j
  *   "dec.x"                [8][d]       f32 decoder residual stream (shared by all slots)
- *   "energy"               [n_samples]  f32 signal energy of the chunk's PCM (wsp_set_token_timestamps); empty before any */
+ *   "energy"               [n_samples]  f32 signal energy of the chunk's PCM (wsp_set_token_timestamps); empty before any
+ *   "pcm"                  [n_samples]  f32 the slot's resident mono PCM (wsp_upload_pcm, or the downmix of wsp_upload_pcm_stereo)
+ *   "pcm_stereo"           [n_frames][2] f32 the slot's stereo pairs (wsp_upload_pcm_stereo); empty after wsp_upload_pcm */
 wsp_status wsp_get_tensor( wsp_context* c, const char* name, int32_t slot, float* dst, size_t cap_floats, size_t* n_floats );
 /* debug: run only the first n encoder layers (negative = all) */
 wsp_status wsp_debug_set_encoder_layers( wsp_context* c, int32_t n );
@@ -372,6 +413,10 @@ wsp_status wsp_test_window_rule( const int32_t rule4[ 4 ], int32_t n_max, int32_
  * energy (n_samples 0). */
 wsp_status wsp_test_token_times( const wsp_token_data* tokens, const float* vlen, int32_t n, int64_t t0, int64_t t1, const int32_t special2[ 2 ],
 	const float* energy, int32_t n_samples, float thold_pt, float thold_ptsum, int64_t state3[ 3 ], wsp_token_time* times );
+/* host only: detectSpeaker's rule (csrc/speaker.h, the code iContext::detectSpeaker and the kernel of wsp_chunk_speakers run) for
+ * segs[n_segs] over interleaved lr[n_frames][2] -> speakers[n_segs], as wsp_chunk_speakers answers them; lr may be NULL when n_frames
+ * is 0 (no stereo) */
+wsp_status wsp_test_speakers( const float* lr, int32_t n_frames, const wsp_segment* segs, int32_t n_segs, int32_t* speakers );
 /* signal_energy_kernel alone over `batch` host clips pcm[b][n_samples[b]] -> energy[b][n_samples[b]] (host); with iters > 0, *ms = the
  * mean time of one launch over `iters` more launches between CUDA events */
 wsp_status wsp_test_signal_energy( int32_t device, const float* const* pcm, const int32_t* n_samples, int32_t batch, float* const* energy,

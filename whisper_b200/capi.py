@@ -51,6 +51,12 @@ SEGMENT_SINGLE = 1          # wsp_window_segments flags
 SEGMENT_PRINT_SPECIAL = 2
 SEGMENT_SPEED_UP = 4
 
+SPEAKER_UNSURE = 0          # wsp_chunk_speakers answers (iContext::detectSpeaker's eSpeakerChannel)
+SPEAKER_LEFT = 1
+SPEAKER_RIGHT = 2
+SPEAKER_NO_STEREO = 255
+SPEAKER_OUT_OF_RANGE = -1   # the segment starts outside the clip (the reference's E_BOUNDS)
+
 
 class ReplicaStats(C.Structure):
     _fields_ = [("device", C.c_int32), ("batches_done", C.c_int32), ("chunks_done", C.c_int32), ("failed", C.c_int32), ("busy_ms", C.c_float), ("load_ms", C.c_float)]
@@ -64,10 +70,11 @@ EXPORTS = [
     "wsp_engine_create", "wsp_engine_create_from_image", "wsp_engine_destroy", "wsp_engine_weight_bytes",
     "wsp_context_create", "wsp_context_destroy", "wsp_synchronize",
     "wsp_context_device_bytes", "wsp_pcm_to_mel", "wsp_pcm_to_mel_window", "wsp_set_mel", "wsp_mel_len", "wsp_get_mel", "wsp_encode", "wsp_set_audio_ctx", "wsp_set_speed_up", "wsp_decode", "wsp_get_logits", "wsp_get_probs",
-    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_run_chunks_until_eot", "wsp_get_chunk_languages", "wsp_run_chunks_window", "wsp_window_segments", "wsp_set_token_timestamps", "wsp_window_token_times", "wsp_upload_pcm", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
+    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_run_chunks_until_eot", "wsp_get_chunk_languages", "wsp_run_chunks_window", "wsp_window_segments", "wsp_set_token_timestamps", "wsp_window_token_times", "wsp_upload_pcm", "wsp_upload_pcm_stereo", "wsp_chunk_speakers", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
     "wsp_host_alloc", "wsp_host_free", "wsp_timings",
     "wsp_replicas_create", "wsp_replicas_count", "wsp_replicas_run_chunks", "wsp_replicas_debug_fail_next", "wsp_replicas_destroy",
     "wsp_test_gemm", "wsp_test_attention", "wsp_test_skinny", "wsp_test_layernorm", "wsp_test_sample", "wsp_test_window_rule", "wsp_test_token_times", "wsp_test_signal_energy",
+    "wsp_test_speakers",
 ]
 
 _lib = None
@@ -142,6 +149,9 @@ def lib():
     sig("wsp_test_token_times", i32, [C.POINTER(TokenData), fp, i32, C.c_int64, C.c_int64, ip, fp, i32, C.c_float, C.c_float,
                                       C.POINTER(C.c_int64), C.POINTER(TokenTime)])
     sig("wsp_upload_pcm", i32, [vp, i32, fp, i32])
+    sig("wsp_upload_pcm_stereo", i32, [vp, i32, fp, i32])
+    sig("wsp_chunk_speakers", i32, [vp, i32, ip, C.POINTER(Segment), ip])
+    sig("wsp_test_speakers", i32, [fp, i32, C.POINTER(Segment), i32, ip])
     sig("wsp_timer_start", i32, [vp])
     sig("wsp_timer_stop", i32, [vp, fp])
     sig("wsp_profile_decode", i32, [vp, i32, i32, fp, ip])
@@ -418,13 +428,24 @@ class Context:
         check(self.L.wsp_set_token_timestamps(self.h, int(on)))
 
     def run_chunks_window(self, pcms, prompt, max_tokens: int = 0, single_segment: bool = False, print_special: bool = False,
-                          batch: int | None = None, token_times: dict | None = None):
+                          batch: int | None = None, token_times: dict | None = None, speakers: bool = False):
         """Each chunk decoded as whisper_full's first window (wsp_run_chunks_window).  pcms: list of float32 arrays, or None to run
         `batch` chunks from the slots' resident PCM (upload_pcm).  Returns (list per chunk of dict(tokens=[token dicts], result=dict,
         segments=[dict(t0, t1, i0, i1, text)]), stage_ms[3]); segment times are doubled while speed-up is on.
         token_times=dict(thold_pt=0.01, thold_ptsum=0.01, max_len=0) (token timestamps must be on): the segments are whisper_full's
         with token_timestamps (wsp_window_token_times), wrapped at max_len characters when max_len > 0; the window's result tokens
-        then carry t0, t1 and vlen, and every segment holds its tokens as `tokens`."""
+        then carry t0, t1 and vlen, and every segment holds its tokens as `tokens`.
+        speakers=True: pcms may hold (n, 2) stereo arrays; every chunk is uploaded to its slot (upload_pcm_stereo, or upload_pcm for
+        a mono one), the batch runs from the resident PCM, and every segment gets "speaker", detectSpeaker's answer for it
+        (chunk_speakers; SPEAKER_NO_STEREO for a mono chunk)."""
+        if speakers and pcms is not None:
+            for b, p in enumerate(pcms):
+                p = np.asarray(p)
+                if p.ndim == 2:
+                    self.upload_pcm_stereo(b, p)
+                else:
+                    self.upload_pcm(b, p)
+            batch, pcms = len(pcms), None
         ptrs, ns = None, None
         if pcms is not None:
             batch = len(pcms)
@@ -451,6 +472,10 @@ class Context:
             else:
                 segs = self._token_times(b, toks, b * cap, res[b], tk, flags, print_special, token_times)
             out.append(dict(tokens=tk, result=result, segments=segs))
+        if speakers:
+            for o, sp in zip(out, self.chunk_speakers([o["segments"] for o in out])):
+                for seg, k in zip(o["segments"], sp):
+                    seg["speaker"] = k
         return out, st
 
     def _token_times(self, b, toks, first, res, tk, flags, print_special, params):
@@ -492,6 +517,26 @@ class Context:
     def upload_pcm(self, slot: int, pcm: np.ndarray):
         pcm = np.ascontiguousarray(pcm, np.float32)
         check(self.L.wsp_upload_pcm(self.h, slot, _f(pcm), pcm.size))
+
+    def upload_pcm_stereo(self, slot: int, lr: np.ndarray):
+        """Interleaved stereo lr[n][2] (left, right) into the slot: kept on the device, and its downmix (l + r) * 0.5 becomes the
+        slot's resident mono PCM (get_tensor("pcm") / "pcm_stereo")."""
+        lr = np.ascontiguousarray(lr, np.float32)
+        if lr.ndim != 2 or lr.shape[1] != 2:
+            raise ValueError("stereo PCM must have shape (n, 2)")
+        check(self.L.wsp_upload_pcm_stereo(self.h, slot, _f(lr), lr.shape[0]))
+
+    def chunk_speakers(self, segments_per_chunk):
+        """detectSpeaker's answer for every segment of chunks [0, len(segments_per_chunk)) against the slots' stereo, in one call of
+        wsp_chunk_speakers: segments are dicts (or objects) with t0 / t1 in 10 ms units.  Returns a list of answer lists (SPEAKER_*)."""
+        counts = [len(s) for s in segments_per_chunk]
+        start = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
+        flat = [seg for s in segments_per_chunk for seg in s]
+        tt = [(seg["t0"], seg["t1"]) if isinstance(seg, dict) else (seg.t0, seg.t1) for seg in flat]
+        segs = (Segment * max(len(flat), 1))(*[Segment(int(a), int(b), 0, 0) for a, b in tt])
+        out = np.zeros(max(len(flat), 1), np.int32)
+        check(self.L.wsp_chunk_speakers(self.h, len(counts), _i(start), segs, _i(out)))
+        return [out[start[b]:start[b + 1]].tolist() for b in range(len(counts))]
 
     def timer_start(self):
         check(self.L.wsp_timer_start(self.h))
@@ -613,6 +658,16 @@ def test_token_times(tokens, vlen, t0: int, t1: int, beg: int, eot: int, energy,
     sp = np.array([beg, eot], np.int32)
     rc = check(lib().wsp_test_token_times(td, _f(vl), n, t0, t1, _i(sp), _f(en), len(energy), thold_pt, thold_ptsum, st, tt))
     return [[int(t.t0), int(t.t1), float(t.vlen)] for t in tt[:n]], [int(x) for x in st], rc == WSP_OK
+
+
+def test_speakers(lr, segments):
+    """csrc/speaker.h on the host: detectSpeaker's answer for each (t0, t1) of `segments` over stereo lr[n][2] (None or an empty
+    array: no stereo)"""
+    a = np.ascontiguousarray(np.zeros((0, 2)) if lr is None else lr, np.float32).reshape(-1, 2)
+    segs = (Segment * max(len(segments), 1))(*[Segment(int(t0), int(t1), 0, 0) for t0, t1 in segments])
+    out = np.zeros(max(len(segments), 1), np.int32)
+    check(lib().wsp_test_speakers(_f(a) if a.size else None, a.shape[0], segs, len(segments), _i(out)))
+    return out[:len(segments)].tolist()
 
 
 def test_signal_energy(pcms, iters: int = 0, device: int = 0):

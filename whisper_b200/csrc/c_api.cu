@@ -1,6 +1,7 @@
 // extern "C" surface (include/whisper_b200.h) + kernel-level test hooks.
 #include "engine.h"
 #include "ref_arith.cuh"
+#include "speaker.h"
 #include "token_times.h"
 #include <algorithm>
 #include <math.h>
@@ -395,6 +396,16 @@ wsp_status wsp_upload_pcm( wsp_context* c, int32_t slot, const float* pcm, int32
 	if( !c ) return fail( WSP_E_POINTER, "context" );
 	return guarded( [ & ]() -> wsp_status { return ctxUploadPcm( *c->c, slot, pcm, n_samples ); } );
 }
+wsp_status wsp_upload_pcm_stereo( wsp_context* c, int32_t slot, const float* lr, int32_t n_frames )
+{
+	if( !c ) return fail( WSP_E_POINTER, "context" );
+	return guarded( [ & ]() -> wsp_status { return ctxUploadPcmStereo( *c->c, slot, lr, n_frames ); } );
+}
+wsp_status wsp_chunk_speakers( wsp_context* c, int32_t batch, const int32_t* seg_start, const wsp_segment* segs, int32_t* speakers )
+{
+	if( !c || !seg_start || !speakers ) return fail( WSP_E_POINTER, "context/seg_start/speakers" );
+	return guarded( [ & ]() -> wsp_status { return ctxChunkSpeakers( *c->c, batch, seg_start, segs, speakers ); } );
+}
 wsp_status wsp_profile_decode( wsp_context* c, int32_t batch, int32_t n_steps, float ms_by_kind[ 4 ], int32_t launches_by_kind[ 4 ] )
 {
 	if( !c || !ms_by_kind || !launches_by_kind ) return fail( WSP_E_POINTER, "context/out" );
@@ -486,6 +497,8 @@ wsp_status wsp_get_tensor( wsp_context* cc, const char* name, int32_t slot, floa
 	}
 	else if( nm == "dec.x" ) { f32 = c.xd; n = (size_t)d * 8; }
 	else if( nm == "energy" ) { f32 = c.energy + (size_t)slot * c.energyCap; n = (size_t)c.energyLen[ (size_t)slot ]; }
+	else if( nm == "pcm" ) { f32 = c.slots[ slot ].pcm; n = (size_t)c.slots[ slot ].pcmSamples; }
+	else if( nm == "pcm_stereo" ) { f32 = c.slots[ slot ].stereo; n = (size_t)2 * c.slots[ slot ].stereoFrames; }
 	else return fail( WSP_E_INVALIDARG, "unknown tensor name " + nm );
 	*n_floats = n;
 	if( !dst ) return WSP_OK;
@@ -764,6 +777,14 @@ wsp_status wsp_test_token_times( const wsp_token_data* tokens, const float* vlen
 	TokenTimeState st{ state3[ 0 ], state3[ 1 ], (int)state3[ 2 ] };
 	if( !computeTokenTimes( tokens, vlen, times, n, t0, t1, special2[ 0 ], special2[ 1 ], energy, n_samples, thold_pt, thold_ptsum, st ) ) return WSP_S_FALSE;
 	state3[ 0 ] = st.tBeg; state3[ 1 ] = st.tLast; state3[ 2 ] = st.tidLast;
+	return WSP_OK;
+}
+
+wsp_status wsp_test_speakers( const float* lr, int32_t n_frames, const wsp_segment* segs, int32_t n_segs, int32_t* speakers )
+{
+	if( ( n_frames > 0 && !lr ) || ( n_segs > 0 && ( !segs || !speakers ) ) ) return fail( WSP_E_POINTER, "lr/segs/speakers" );
+	if( n_frames < 0 || n_segs < 0 ) return fail( WSP_E_INVALIDARG, "n_frames / n_segs" );
+	for( int32_t i = 0; i < n_segs; i++ ) speakers[ i ] = speakerOfSegment( lr, n_frames, segs[ i ].t0, segs[ i ].t1 );
 	return WSP_OK;
 }
 

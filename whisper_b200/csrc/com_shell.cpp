@@ -10,6 +10,7 @@
 #include "../../include/whisper_b200_com.h"
 #include "pcm_streamer.h"
 #include "capture_loop.h"
+#include "speaker.h"
 #include "wav_reader.h"
 #include "token_times.h"
 #include "window_rule.h"
@@ -521,26 +522,10 @@ namespace
 			}
 			const int64_t begin = ( ( (int64_t)time.begin.ticks - results.timeOffset ) * 100 ) / 10000000;   // 10 ms chunks, :9-13
 			const int64_t end = ( ( (int64_t)time.end.ticks - results.timeOffset ) * 100 ) / 10000000;
-			if( end - begin <= 0 ) return S_OK;
-			if( !curStereo )
-			{
-				result = eSpeakerChannel::NoStereoData;
-				return S_OK;
-			}
-			const uint64_t first = (uint64_t)begin * 160, count = (uint64_t)( end - begin ) * 160;       // Spectrogram::copyStereoPcm, Spectrogram.cpp:142-168
-			if( begin < 0 || first >= curStereoFrames ) return E_BOUNDS;
-			const uint64_t n = std::min<uint64_t>( count, curStereoFrames - first );                     // the rest of the slice is zero: adds nothing
-			// the reference adds two stereo samples per step into four f32 lanes and folds them at the end (:26-50); same order here
-			float accL[ 2 ] = { 0, 0 }, accR[ 2 ] = { 0, 0 };
-			const float* p = curStereo + 2 * first;
-			for( uint64_t i = 0; i < n; i++ )
-			{
-				accL[ i & 1 ] += fabsf( p[ 2 * i ] );
-				accR[ i & 1 ] += fabsf( p[ 2 * i + 1 ] );
-			}
-			const float left = accL[ 0 ] + accL[ 1 ], right = accR[ 0 ] + accR[ 1 ];
-			const uint32_t mask = ( left > right * 1.1f ? 1u : 0u ) | ( right > left * 1.1f ? 2u : 0u );   // :53-71
-			result = (eSpeakerChannel)mask;
+			// the rule (csrc/speaker.h) is the one wsp_chunk_speakers runs on the device
+			const int r = wsp::speakerOfSegment( curStereo, curStereo ? (int64_t)curStereoFrames : 0, begin, end );
+			if( r == WSP_SPEAKER_OUT_OF_RANGE ) return E_BOUNDS;   // Spectrogram::copyStereoPcm, Spectrogram.cpp:142-168
+			result = (eSpeakerChannel)(uint8_t)r;
 			return S_OK;
 		}
 		HRESULT WSPCALL getModel( iModel** pp ) override;

@@ -2,6 +2,7 @@
 // Reference: WhisperContext::encode / ::decode (Whisper/Whisper/WhisperContext.cpp:310-388, 578-639); oracle whisper_encode /
 // whisper_decode (Whisper/source/whisper.cpp:1084-1872).  All launches go to one stream; the N = 1 decoder step is a CUDA graph.
 #include "engine.h"
+#include "speaker.h"
 #include <algorithm>
 #include <math.h>
 #include <memory>
@@ -35,11 +36,11 @@ namespace wsp
 	{
 		if( e ) cudaSetDevice( e->device );
 		if( stepGraph ) cudaGraphExecDestroy( stepGraph );
-		for( auto& s : slots ) { if( s.mel ) cudaFree( s.mel ); if( s.pcm ) cudaFree( s.pcm ); }
+		for( auto& s : slots ) { if( s.mel ) cudaFree( s.mel ); if( s.pcm ) cudaFree( s.pcm ); if( s.stereo ) cudaFree( s.stereo ); }
 		for( auto& v : prof.pool ) cudaEventDestroy( v );
 		for( auto& v : timerEv ) if( v ) cudaEventDestroy( v );
 		void* bufs[] = { stepLayers, flowBias, flowExch, flowCtrl, megaBarrier, stepMarks, melMax, pcmDev, melF16, conv1, x, xn, q, k, vt, attn, h, crossK, crossV, selfK, selfV, xd, qd, attnD, hD, logits, probs, tieScratch,
-			tokensDev, dNPast, sampled, history, endStep, langIds, langProbs, winCtl, winState, tokenLog, energy };
+			tokensDev, dNPast, sampled, history, endStep, langIds, langProbs, winCtl, winState, tokenLog, energy, speakerBuf };
 		for( void* b : bufs ) if( b ) cudaFree( b );
 		if( nEndedHost ) cudaFreeHost( nEndedHost );
 		if( energyHost ) cudaFreeHost( energyHost );
@@ -749,7 +750,82 @@ namespace wsp
 			s.pcmCap = nSamples;
 		}
 		s.pcmSamples = nSamples;
+		s.stereoFrames = 0;
 		WSP_CUDA( cudaMemcpyAsync( s.pcm, pcmHost, (size_t)nSamples * 4, cudaMemcpyHostToDevice, c.stream ) );
+		WSP_CUDA( cudaStreamSynchronize( c.stream ) );
+		return WSP_OK;
+	}
+
+	// the stereo pairs into the slot, and their downmix as its resident mono PCM
+	int ctxUploadPcmStereo( Context& c, int slot, const float* lrHost, int nFrames )
+	{
+		if( slot < 0 || slot >= c.maxB ) return fail( WSP_E_BOUNDS, "chunk slot out of range" );
+		if( ( !lrHost && nFrames != 0 ) || nFrames < 0 ) return fail( WSP_E_INVALIDARG, "pcm" );
+		WSP_CUDA( cudaSetDevice( c.e->device ) );
+		MelSlot& s = c.slots[ slot ];
+		if( nFrames > s.stereoCap )
+		{
+			if( s.stereo ) { WSP_CUDA( cudaStreamSynchronize( c.stream ) ); cudaFree( s.stereo ); s.stereo = nullptr; }
+			c.devBytes -= (uint64_t)s.stereoCap * 8;
+			s.stereoCap = 0;
+			WSP_CHECK( devAlloc( s.stereo, (size_t)2 * nFrames ) );
+			c.devBytes += (uint64_t)nFrames * 8;
+			s.stereoCap = nFrames;
+		}
+		if( nFrames > s.pcmCap )
+		{
+			if( s.pcm ) { WSP_CUDA( cudaStreamSynchronize( c.stream ) ); cudaFree( s.pcm ); s.pcm = nullptr; }
+			WSP_CHECK( devAlloc( s.pcm, (size_t)nFrames ) );
+			s.pcmCap = nFrames;
+		}
+		s.pcmSamples = nFrames;
+		s.stereoFrames = nFrames;
+		if( nFrames > 0 ) WSP_CUDA( cudaMemcpyAsync( s.stereo, lrHost, (size_t)nFrames * 8, cudaMemcpyHostToDevice, c.stream ) );
+		WSP_CUDA( kern::downmixStereo( s.stereo, s.pcm, nFrames, c.stream ) );
+		launched();
+		WSP_CUDA( cudaStreamSynchronize( c.stream ) );
+		return WSP_OK;
+	}
+
+	// detectSpeaker for every segment of a batch: speakerSpan on the host picks each segment's frames (or its answer), then one launch
+	// folds and decides them all between one copy in and one copy out
+	int ctxChunkSpeakers( Context& c, int batch, const int32_t* segStart, const wsp_segment* segs, int32_t* speakers )
+	{
+		if( batch < 1 || batch > c.maxB ) return fail( WSP_E_BOUNDS, "batch exceeds the context's max_batch" );
+		if( segStart[ 0 ] != 0 ) return fail( WSP_E_INVALIDARG, "seg_start[0] must be 0" );
+		for( int b = 0; b < batch; b++ )
+			if( segStart[ b + 1 ] < segStart[ b ] ) return fail( WSP_E_INVALIDARG, "seg_start decreases" );
+		const size_t n = (size_t)segStart[ batch ];
+		if( n == 0 ) return WSP_OK;
+		if( !segs ) return fail( WSP_E_POINTER, "segs" );
+		std::vector<kern::SpeakerJob> jobs( n );
+		for( int b = 0; b < batch; b++ )
+		{
+			const MelSlot& s = c.slots[ b ];
+			for( int32_t i = segStart[ b ]; i < segStart[ b + 1 ]; i++ )
+			{
+				int64_t first = 0, count = 0;
+				const int pre = speakerSpan( segs[ i ].t0, segs[ i ].t1, s.stereoFrames, first, count );
+				jobs[ (size_t)i ] = kern::SpeakerJob{ pre == kSpeakerSums ? s.stereo + 2 * first : nullptr, count, pre, 0 };
+			}
+		}
+		WSP_CUDA( cudaSetDevice( c.e->device ) );
+		const size_t outOffset = ( n * sizeof( kern::SpeakerJob ) + 15 ) & ~(size_t)15;
+		if( n > c.speakerCap )
+		{
+			if( c.speakerBuf ) { WSP_CUDA( cudaStreamSynchronize( c.stream ) ); cudaFree( c.speakerBuf ); c.speakerBuf = nullptr; }
+			c.devBytes -= (uint64_t)c.speakerCap * ( sizeof( kern::SpeakerJob ) + 4 );
+			c.speakerCap = 0;
+			WSP_CHECK( devAlloc( c.speakerBuf, outOffset + n * 4 ) );
+			c.devBytes += (uint64_t)n * ( sizeof( kern::SpeakerJob ) + 4 );
+			c.speakerCap = n;
+		}
+		kern::SpeakerJob* dJobs = reinterpret_cast<kern::SpeakerJob*>( c.speakerBuf );
+		int32_t* dOut = reinterpret_cast<int32_t*>( c.speakerBuf + outOffset );
+		WSP_CUDA( cudaMemcpyAsync( dJobs, jobs.data(), n * sizeof( kern::SpeakerJob ), cudaMemcpyHostToDevice, c.stream ) );
+		WSP_CUDA( kern::chunkSpeakers( dJobs, dOut, (int)n, c.stream ) );
+		launched();
+		WSP_CUDA( cudaMemcpyAsync( speakers, dOut, n * 4, cudaMemcpyDeviceToHost, c.stream ) );
 		WSP_CUDA( cudaStreamSynchronize( c.stream ) );
 		return WSP_OK;
 	}

@@ -97,6 +97,9 @@ namespace wsp
 		float* pcm = nullptr;   // optional device-resident PCM (wsp_upload_pcm), for the HBM-resident bench leg
 		int pcmCap = 0;
 		int pcmSamples = 0;
+		float* stereo = nullptr;   // [stereoCap][2] interleaved pairs of wsp_upload_pcm_stereo, whose downmix is `pcm`
+		int stereoCap = 0;
+		int stereoFrames = 0;      // 0: the slot has no stereo (wsp_upload_pcm drops it)
 	};
 
 	// per-kernel-kind device time of the decoder, collected by an instrumented (un-graphed) pass: wsp_profile_decode
@@ -192,6 +195,9 @@ namespace wsp
 		std::vector<int> energyLen;     // [maxB] samples of each slot's device energy
 		int windowEnergyBatch = 0;      // batch of the last wsp_run_chunks_window call if it computed the energy, else 0
 		std::vector<int> windowEnergyLen;   // [that batch] samples of each chunk's energy in energyHost
+		// wsp_chunk_speakers: the segments' jobs, then their answers, in one device buffer
+		uint8_t* speakerBuf = nullptr;
+		size_t speakerCap = 0;          // segments it holds
 		int lastLogitRows = 0;
 		int nPastHost = 0;              // host mirror of the device-resident n_past (it advances on the device between graph replays)
 		int debugEncLayers = -1;
@@ -246,6 +252,8 @@ namespace wsp
 	int ctxSetTokenTimestamps( Context& c, int on );
 	int ctxDecode( Context& c, const int32_t* tokensHost, int nTokens, int nPast, int batch, uint32_t flags, wsp_token_data* sampledHost );
 	int ctxUploadPcm( Context& c, int slot, const float* pcmHost, int nSamples );
+	int ctxUploadPcmStereo( Context& c, int slot, const float* lrHost, int nFrames );
+	int ctxChunkSpeakers( Context& c, int batch, const int32_t* segStart, const wsp_segment* segs, int32_t* speakers );
 	int ctxProfileDecode( Context& c, int batch, int nSteps, float* msByKind, int* launchesByKind );
 	// wsp_run_chunks_window's outputs
 	struct WindowOut

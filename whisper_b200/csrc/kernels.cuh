@@ -74,6 +74,21 @@ namespace kern
 	};
 	cudaError_t signalEnergy( const EnergyBatch& eb, cudaStream_t s );
 
+	// ---- stereo chunks and their speakers (wsp_upload_pcm_stereo, wsp_chunk_speakers) -------------------------------------------
+	// mono[i] = (lr[2i] + lr[2i+1]) * 0.5f for i < nFrames (AudioBuffer::appendDownmixedStereo); one launch, also for nFrames = 0
+	cudaError_t downmixStereo( const float* lr, float* mono, int nFrames, cudaStream_t s );
+	// one segment of detectSpeaker (speaker.h): pre != wsp::kSpeakerSums is the answer already; otherwise the lane sums of the count
+	// frames at lr (16-byte aligned) decide it
+	struct SpeakerJob
+	{
+		const float* lr;
+		int64_t count;
+		int32_t pre;
+		int32_t pad;
+	};
+	// out[i] = the answer of jobs[i] for i < n, one warp per segment; n >= 1
+	cudaError_t chunkSpeakers( const SpeakerJob* jobs, int32_t* out, int n, cudaStream_t s );
+
 	// ---- LayerNorm + affine -> f16 (a5, a11) -------------------------------------------------------------------------
 	cudaError_t layerNormF16( const float* x, const float* gamma, const float* beta, __half* out, int rows, int d, cudaStream_t s );
 

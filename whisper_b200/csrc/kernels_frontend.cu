@@ -1,6 +1,7 @@
 // Front-end + normalisation kernels (HBM/latency-bound, no tensor cores): log-mel spectrogram, window gather, LayerNorm, embedding.
 #include "kernels.cuh"
 #include "ptx.cuh"
+#include "speaker.h"
 #include <math.h>
 
 namespace kern
@@ -256,6 +257,95 @@ namespace kern
 		for( int b = 0; b < eb.count; b++ ) maxN = eb.nSamples[ b ] > maxN ? eb.nSamples[ b ] : maxN;
 		const int tiles = ( maxN + ENERGY_TILE - 1 ) / ENERGY_TILE;   // one launch even for a batch of empty clips
 		signal_energy_kernel<<<dim3( tiles > 0 ? tiles : 1, eb.count ), ENERGY_TILE, 0, s>>>( eb );
+		return cudaGetLastError();
+	}
+
+	// ---------------------------------------------------------------------------------------------------------------
+	// stereo -> mono (AudioBuffer::appendDownmixedStereo, Whisper/MF/AudioBuffer.cpp:57-93): (l + r) * 0.5f per frame, two frames per
+	// thread and step.  An add then a multiply cannot contract into an FMA, so every sample is the reference's bit for bit.
+	constexpr int DOWNMIX_THREADS = 256;
+	__global__ void __launch_bounds__( DOWNMIX_THREADS )
+		downmix_stereo_kernel( const float* __restrict__ lr, float* __restrict__ mono, int nFrames )
+	{
+		const float4* in = reinterpret_cast<const float4*>( lr );
+		float2* out = reinterpret_cast<float2*>( mono );
+		for( int i = blockIdx.x * blockDim.x + threadIdx.x; i < nFrames / 2; i += gridDim.x * blockDim.x )
+		{
+			const float4 v = in[ i ];
+			out[ i ] = make_float2( ( v.x + v.y ) * 0.5f, ( v.z + v.w ) * 0.5f );
+		}
+		if( ( nFrames & 1 ) && blockIdx.x == 0 && threadIdx.x == 0 ) mono[ nFrames - 1 ] = ( lr[ 2 * nFrames - 2 ] + lr[ 2 * nFrames - 1 ] ) * 0.5f;
+	}
+	cudaError_t downmixStereo( const float* lr, float* mono, int nFrames, cudaStream_t s )
+	{
+		const int blocks = ( nFrames / 2 + DOWNMIX_THREADS - 1 ) / DOWNMIX_THREADS;
+		downmix_stereo_kernel<<<blocks > 0 ? blocks : 1, DOWNMIX_THREADS, 0, s>>>( lr, mono, nFrames );
+		return cudaGetLastError();
+	}
+
+	// ---------------------------------------------------------------------------------------------------------------
+	// detectSpeaker's channel sums (ContextImpl.diarize.cpp:17-52): one warp per segment.  The reference keeps four f32 chains, one per
+	// SSE lane { |L even|, |R even|, |L odd|, |R odd| }, each added in frame order; a tree would round differently and move decisions
+	// whose ratio lies within rounding of 1.1.  So lanes 0..3 of the warp each run one chain over a frame pair (one float4) per step,
+	// and the whole warp keeps SPK_STAGES - 1 tiles of pairs in flight with coalesced cp.async copies into shared memory, so the chains
+	// never wait for HBM.  Pairs past the segment, and the missing odd frame of an odd count, are zero-filled: +0 leaves a chain as it is.
+	constexpr int SPK_WARPS = 4;
+	constexpr int SPK_STAGES = 3;
+	constexpr int SPK_PER_LANE = 8;
+	constexpr int SPK_TILE = 32 * SPK_PER_LANE;   // frame pairs per stage
+	static_assert( SPK_WARPS * SPK_STAGES * SPK_TILE * 16 <= 48 * 1024, "static shared memory" );
+	__global__ void __launch_bounds__( SPK_WARPS * 32 )
+		speaker_kernel( const SpeakerJob* __restrict__ jobs, int32_t* __restrict__ out, int n )
+	{
+		__shared__ float4 tiles[ SPK_WARPS ][ SPK_STAGES ][ SPK_TILE ];
+		const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+		const int seg = blockIdx.x * SPK_WARPS + warp;
+		if( seg >= n ) return;
+		const SpeakerJob job = jobs[ seg ];
+		if( job.pre != wsp::kSpeakerSums )
+		{
+			if( lane == 0 ) out[ seg ] = job.pre;
+			return;
+		}
+		const float4* src = reinterpret_cast<const float4*>( job.lr );
+		const int64_t count = job.count;
+		const int nTiles = (int)( ( ( count + 1 ) / 2 + SPK_TILE - 1 ) / SPK_TILE );
+		float4( *buf )[ SPK_TILE ] = tiles[ warp ];
+		auto stage = [ & ]( int t ) {
+			if( t < nTiles )
+#pragma unroll
+				for( int k = 0; k < SPK_PER_LANE; k++ )
+				{
+					const int64_t p = (int64_t)t * SPK_TILE + k * 32 + lane;
+					const uint32_t bytes = 2 * p + 2 <= count ? 16u : ( 2 * p < count ? 8u : 0u );
+					ptx::cp_async16_zfill( &buf[ t % SPK_STAGES ][ k * 32 + lane ], bytes ? src + p : src, bytes );
+				}
+			ptx::cp_async_commit();   // an empty group past the last tile keeps the wait count below uniform
+		};
+#pragma unroll
+		for( int t = 0; t < SPK_STAGES - 1; t++ ) stage( t );
+		float acc = 0.0f;   // lane c < 4: lane c of the reference's accumulator
+		for( int t = 0; t < nTiles; t++ )
+		{
+			stage( t + SPK_STAGES - 1 );                 // into the buffer folded in step t - 1
+			ptx::cp_async_wait<SPK_STAGES - 1>();
+			__syncwarp();
+			if( lane < 4 )
+			{
+				const float* f = reinterpret_cast<const float*>( buf[ t % SPK_STAGES ] ) + lane;
+#pragma unroll 32
+				for( int j = 0; j < SPK_TILE; j++ ) acc = wsp::speakerFold( acc, f[ 4 * j ] );
+			}
+			__syncwarp();
+		}
+		const float lEven = __shfl_sync( 0xFFFFFFFFu, acc, 0 ), rEven = __shfl_sync( 0xFFFFFFFFu, acc, 1 );
+		const float lOdd = __shfl_sync( 0xFFFFFFFFu, acc, 2 ), rOdd = __shfl_sync( 0xFFFFFFFFu, acc, 3 );
+		if( lane == 0 ) out[ seg ] = wsp::speakerDecide( lEven, rEven, lOdd, rOdd );
+	}
+	cudaError_t chunkSpeakers( const SpeakerJob* jobs, int32_t* out, int n, cudaStream_t s )
+	{
+		if( n < 1 ) return cudaErrorInvalidValue;
+		speaker_kernel<<<( n + SPK_WARPS - 1 ) / SPK_WARPS, SPK_WARPS * 32, 0, s>>>( jobs, out, n );
 		return cudaGetLastError();
 	}
 

@@ -199,8 +199,14 @@ namespace ptx
 	{
 		asm volatile( "cp.async.cg.shared.global [%0], [%1], 16;" ::"r"( smem_u32( smemDst ) ), "l"( gmemSrc ) : "memory" );
 	}
+	// the same with only the first srcBytes (0..16) read and the rest of the 16 bytes zero-filled
+	__device__ __forceinline__ void cp_async16_zfill( void* smemDst, const void* gmemSrc, uint32_t srcBytes )
+	{
+		asm volatile( "cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"( smem_u32( smemDst ) ), "l"( gmemSrc ), "r"( srcBytes ) : "memory" );
+	}
 	__device__ __forceinline__ void cp_async_commit() { asm volatile( "cp.async.commit_group;" ::: "memory" ); }
 	__device__ __forceinline__ void cp_async_wait_all() { asm volatile( "cp.async.wait_group 0;" ::: "memory" ); }
+	template<int N> __device__ __forceinline__ void cp_async_wait() { asm volatile( "cp.async.wait_group %0;" ::"n"( N ) : "memory" ); }
 
 	// nanoseconds of the global timer (debug marks, and the time limit of spin waits)
 	__device__ __forceinline__ unsigned long long globaltimer()
