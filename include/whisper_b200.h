@@ -21,6 +21,7 @@
  *   wsp_run_chunks_until_eot  the same loop, each chunk cut at its first EOT and the batch stopped soon after its last one
  *   wsp_get_chunk_languages   whisper_lang_auto_detect (Whisper/source/whisper.cpp:2428-2495) per chunk of a run_chunks* call
  *   wsp_run_chunks_window     the same loop, each chunk decoded and ended as whisper_full's first window (whisper.cpp:2910-3003)
+ *   wsp_run_spans_window      the same, each row whisper_full's first window at a span's offset_ms / duration_ms (whisper.cpp:2810-2818)
  *   wsp_window_segments       whisper_full's segments of one window (whisper.cpp:3026-3119)
  *   wsp_set_token_timestamps  whisper_full_params::token_timestamps (Whisper/API/sFullParams.h eFullParamsFlags::TokenTimestamps): the
  *                             signal energy of get_signal_energy (whisper.cpp:3356-3372), computed on the device
@@ -231,6 +232,35 @@ typedef struct wsp_window_result
 wsp_status wsp_run_chunks_window( wsp_context* c, const float* const* pcm, const int32_t* n_samples, int32_t batch, const int32_t* prompt,
 	int32_t n_prompt, const wsp_window_params* params, wsp_token_data* tokens_out, int32_t cap, wsp_window_result* results, float* stage_ms );
 
+/* A time interval of a resident clip: whisper_full_params::offset_ms and duration_ms (sFullParams.h:51-52) of slot `slot`'s PCM. */
+typedef struct wsp_window_span
+{
+	int32_t slot;             /* the source: the slot's resident PCM (wsp_upload_pcm, or the downmix of wsp_upload_pcm_stereo) */
+	int32_t offset_ms;        /* >= 0 */
+	int32_t duration_ms;      /* 0: to the end of the clip; < 0: no window, as in the reference */
+} wsp_window_span;
+/* wsp_run_chunks_window over spans: row b is the first window of whisper_full( the clip of spans[b].slot, offset_ms, duration_ms ) with
+ * no past prompt (whisper.cpp:2810-2818, 2910-3003).  With n_len = the whole clip's mel length (n_samples / 160, or / 320 under
+ * speed-up), seek = offset_ms / 10 and seek_end = seek + (duration_ms == 0 ? n_len : duration_ms / 10):
+ *   - a row with seek_end <= seek + 100 runs no window (:2816, 2871): its result is all zeros;
+ *   - the row's encode reads frames [seek, seek + 2n) of the source's whole-clip log-mel, normalised over the whole clip, frames past
+ *     n_len zero (:1112-1120): the encoder sees the audio past seek_end, as the reference's does;
+ *   - the window rule runs at seek over seek_end, and wsp_window_segments( ..., seek, ... ) gives the row's segments at absolute times
+ *     in the clip (:3028, 3042).
+ * Under speed-up seek and seek_end count frames at the vocoder's hop of 320 samples, as in the reference: an offset then lands at twice
+ * its time in the clip, and segment times are doubled.  Rows naming one slot share its log-mel, and its signal energy while token
+ * timestamps are on: each named slot's are computed once per call, in the batched launches of wsp_run_chunks_window, and a slot no row
+ * names is not touched.  WSP_TOKEN_LANGUAGE_AUTO detects each row's language from the row's own encode, as whisper_lang_auto_detect(
+ * offset_ms ) does (:2428-2495); whisper_full itself detects at offset 0 whatever offset_ms is (:2792), so a row gets the language
+ * spoken in its span.  Every row keeps the one caller prompt and n_past.  Outputs, cap, stage_ms, audio_ctx and the other settings are
+ * those of wsp_run_chunks_window.  Every argument is checked before anything is enqueued, and an error launches nothing: a null
+ * pointer is WSP_E_POINTER (tokens_out and stage_ms may be NULL); a batch outside [1, max_batch] or a slot outside max_batch
+ * WSP_E_BOUNDS; a slot without resident PCM, a negative offset_ms (undefined in the reference, which reads before the mel) or the
+ * sentinel on a row whose seek is at or past its source's n_len (the reference's -2, :2440-2443) WSP_E_INVALIDARG.  The seek
+ * arithmetic cannot overflow int32: each of its terms is below 2^31 / 10. */
+wsp_status wsp_run_spans_window( wsp_context* c, const wsp_window_span* spans, int32_t batch, const int32_t* prompt, int32_t n_prompt,
+	const wsp_window_params* params, wsp_token_data* tokens_out, int32_t cap, wsp_window_result* results, float* stage_ms );
+
 /* segmentation flags */
 enum
 {
@@ -270,10 +300,14 @@ typedef struct wsp_token_time_params
 	float thold_ptsum;        /* whisper_full_params::thold_ptsum (default 0.01) */
 	int32_t max_len;          /* whisper_full_params::max_len: wrap segments at this many characters (<= 0: no wrapping) */
 } wsp_token_time_params;
-/* Host only: chunk `chunk`'s segments of this context's last wsp_run_chunks_window call as whisper_full emits them with
- * token_timestamps on.  tokens and result are that call's for the chunk, flags as for wsp_window_segments.  The window is cut by
- * wsp_window_segments; then, segment by segment in order and from the state whisper_full starts a call with, the token times of
- * whisper.cpp:3374-3600 run over the chunk's signal energy, and with max_len > 0 each segment is wrapped right after its token
+/* Host only: chunk `chunk`'s segments of this context's last wsp_run_chunks_window or wsp_run_spans_window call as whisper_full emits
+ * them with token_timestamps on.  tokens and result are that call's for the chunk, flags as for wsp_window_segments.  The window is
+ * cut by wsp_window_segments at the chunk's seek (0, or a span's offset_ms / 10, so times are absolute in the clip); then, segment by
+ * segment in order and from the state whisper_full starts a call with (t_beg = t_last = 0, :2803-2808), the token times of
+ * whisper.cpp:3374-3600 run over the signal energy of the chunk's whole clip, clamped at its last sample (:3320-3322): a span's first
+ * segment that does not open with beg reads energy before the span.  A spans call keeps each source's energy in the row of its slot
+ * of [max_batch][longest clip] f32 on the device and again in pinned host memory, so an hour-long source costs
+ * max_batch x 57.6 M samples x 4 B in each.  With max_len > 0 each segment is wrapped right after its token
  * times (:3063-3070, 3107-3114).  Under WSP_SEGMENT_SPEED_UP this is what the reference does: segment times are doubled, the
  * timestamp token times t_beg + 2 (tid - beg) are not, and the energy is that of the original samples.  segs receives the segments
  * after wrapping, the first min(*n_segs, cap) of them (a segment's text is that of its non-special tokens once wrapped);

@@ -35,6 +35,10 @@ class WindowResult(C.Structure):
     _fields_ = [("n_sampled", C.c_int32), ("n_tokens", C.c_int32), ("seek_delta", C.c_int32), ("failed", C.c_int32)]
 
 
+class WindowSpan(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("offset_ms", C.c_int32), ("duration_ms", C.c_int32)]
+
+
 class Segment(C.Structure):
     _fields_ = [("t0", C.c_int64), ("t1", C.c_int64), ("i0", C.c_int32), ("i1", C.c_int32)]
 
@@ -70,7 +74,7 @@ EXPORTS = [
     "wsp_engine_create", "wsp_engine_create_from_image", "wsp_engine_destroy", "wsp_engine_weight_bytes",
     "wsp_context_create", "wsp_context_destroy", "wsp_synchronize",
     "wsp_context_device_bytes", "wsp_pcm_to_mel", "wsp_pcm_to_mel_window", "wsp_set_mel", "wsp_mel_len", "wsp_get_mel", "wsp_encode", "wsp_set_audio_ctx", "wsp_set_speed_up", "wsp_decode", "wsp_get_logits", "wsp_get_probs",
-    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_run_chunks_until_eot", "wsp_get_chunk_languages", "wsp_run_chunks_window", "wsp_window_segments", "wsp_set_token_timestamps", "wsp_window_token_times", "wsp_upload_pcm", "wsp_upload_pcm_stereo", "wsp_chunk_speakers", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
+    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_run_chunks_until_eot", "wsp_get_chunk_languages", "wsp_run_chunks_window", "wsp_run_spans_window", "wsp_window_segments", "wsp_set_token_timestamps", "wsp_window_token_times", "wsp_upload_pcm", "wsp_upload_pcm_stereo", "wsp_chunk_speakers", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
     "wsp_host_alloc", "wsp_host_free", "wsp_timings",
     "wsp_replicas_create", "wsp_replicas_count", "wsp_replicas_run_chunks", "wsp_replicas_debug_fail_next", "wsp_replicas_destroy",
     "wsp_test_gemm", "wsp_test_attention", "wsp_test_skinny", "wsp_test_layernorm", "wsp_test_sample", "wsp_test_window_rule", "wsp_test_token_times", "wsp_test_signal_energy",
@@ -140,6 +144,8 @@ def lib():
     sig("wsp_get_chunk_languages", i32, [vp, i32, ip, fp, sz])
     sig("wsp_run_chunks_window", i32, [vp, C.POINTER(fp), ip, i32, ip, i32, C.POINTER(WindowParams), C.POINTER(TokenData), i32,
                                        C.POINTER(WindowResult), fp])
+    sig("wsp_run_spans_window", i32, [vp, C.POINTER(WindowSpan), i32, ip, i32, C.POINTER(WindowParams), C.POINTER(TokenData), i32,
+                                      C.POINTER(WindowResult), fp])
     sig("wsp_window_segments", i32, [vp, C.POINTER(TokenData), C.POINTER(WindowResult), i32, u32, C.POINTER(Segment), i32, ip])
     sig("wsp_test_window_rule", i32, [ip, i32, i32, i32, ip, i32, ip, ip])
     sig("wsp_set_token_timestamps", i32, [vp, i32])
@@ -460,23 +466,51 @@ class Context:
         prm = WindowParams(int(max_tokens), int(bool(single_segment)))
         check(self.L.wsp_run_chunks_window(self.h, ptrs, None if ns is None else _i(ns), batch, _i(pr), pr.size, C.byref(prm), toks, cap,
                                            res, _f(st)))
+        out = self._windows(toks, cap, res, list(range(batch)), [0] * batch, single_segment, print_special, token_times, speakers)
+        return out, st
+
+    def run_spans_window(self, spans, prompt, max_tokens: int = 0, single_segment: bool = False, print_special: bool = False,
+                         token_times: dict | None = None, speakers: bool = False):
+        """Row b decoded as the first window of whisper_full( clip of slot spans[b][0], offset_ms, duration_ms ) (wsp_run_spans_window):
+        spans = [(slot, offset_ms, duration_ms)] over the slots' resident PCM (upload_pcm / upload_pcm_stereo).  Returns what
+        run_chunks_window returns, one entry per row, with segment times absolute in the clip (doubled while speed-up is on).
+        speakers=True: every segment gets "speaker", detectSpeaker's answer for it against its row's slot's stereo."""
+        batch = len(spans)
+        sp = (WindowSpan * max(batch, 1))(*[WindowSpan(int(s), int(o), int(d)) for s, o, d in spans])
+        pr = np.ascontiguousarray(prompt, np.int32)
+        cap = self.model.n_text_ctx // 2 - 4
+        toks = (TokenData * (max(batch, 1) * cap))()
+        res = (WindowResult * max(batch, 1))()
+        st = np.zeros(3, np.float32)
+        prm = WindowParams(int(max_tokens), int(bool(single_segment)))
+        check(self.L.wsp_run_spans_window(self.h, sp, batch, _i(pr), pr.size, C.byref(prm), toks, cap, res, _f(st)))
+        out = self._windows(toks, cap, res, [int(s) for s, _o, _d in spans], [int(o) // 10 for _s, o, _d in spans], single_segment,
+                            print_special, token_times, speakers)
+        return out, st
+
+    def _windows(self, toks, cap, res, slots, seeks, single_segment, print_special, token_times, speakers):
+        """the per-row dicts of a window call: row b's window ran at seeks[b] over slots[b]'s clip"""
         flags = ((SEGMENT_SINGLE if single_segment else 0) | (SEGMENT_PRINT_SPECIAL if print_special else 0)
                  | (SEGMENT_SPEED_UP if self.speed_up else 0))
         out = []
-        for b in range(batch):
+        for b, seek in enumerate(seeks):
             r = res[b]
             result = dict(n_sampled=r.n_sampled, n_tokens=r.n_tokens, seek_delta=r.seek_delta, failed=r.failed)
             tk = [dict(id=t.id, tid=t.tid, p=t.p, pt=t.pt, ptsum=t.ptsum) for t in toks[b * cap:b * cap + r.n_sampled]]
             if token_times is None:
-                segs = self.model.window_segments(tk, result, 0, flags)
+                segs = self.model.window_segments(tk, result, seek, flags)
             else:
                 segs = self._token_times(b, toks, b * cap, res[b], tk, flags, print_special, token_times)
             out.append(dict(tokens=tk, result=result, segments=segs))
         if speakers:
-            for o, sp in zip(out, self.chunk_speakers([o["segments"] for o in out])):
-                for seg, k in zip(o["segments"], sp):
+            # wsp_chunk_speakers reads chunk k's segments against slot k's stereo: the rows' segments grouped by slot
+            by_slot = [[] for _ in range(max(slots) + 1)]
+            for o, s in zip(out, slots):
+                by_slot[s] += o["segments"]
+            for segs, sp in zip(by_slot, self.chunk_speakers(by_slot)):
+                for seg, k in zip(segs, sp):
                     seg["speaker"] = k
-        return out, st
+        return out
 
     def _token_times(self, b, toks, first, res, tk, flags, print_special, params):
         p = dict(thold_pt=0.01, thold_ptsum=0.01, max_len=0)

@@ -327,6 +327,17 @@ wsp_status wsp_run_chunks_window( wsp_context* c, const float* const* pcm, const
 		return ctxRunChunks( *c->c, pcm, n_samples, batch, prompt, n_prompt, nMax, nullptr, nullptr, stage_ms, pcm == nullptr, &w );
 	} );
 }
+wsp_status wsp_run_spans_window( wsp_context* c, const wsp_window_span* spans, int32_t batch, const int32_t* prompt, int32_t n_prompt,
+	const wsp_window_params* params, wsp_token_data* tokens_out, int32_t cap, wsp_window_result* results, float* stage_ms )
+{
+	if( !c ) return fail( WSP_E_POINTER, "context" );
+	if( !spans || !prompt || !params || !results ) return fail( WSP_E_POINTER, "spans/prompt/params/results" );
+	return guarded( [ & ]() -> wsp_status {
+		const WindowOut w{ *params, tokens_out, cap, results };
+		const int nMax = c->c->e->hp.n_text_ctx / 2 - 4;                                             // whisper.cpp:2926
+		return ctxRunSpans( *c->c, spans, batch, prompt, n_prompt, nMax, stage_ms, w );
+	} );
+}
 wsp_status wsp_window_segments( const wsp_model* m, const wsp_token_data* tokens, const wsp_window_result* result, int32_t seek,
 	uint32_t flags, wsp_segment* segs, int32_t cap, int32_t* n_segs )
 {
@@ -346,14 +357,15 @@ wsp_status wsp_window_token_times( wsp_context* c, int32_t chunk, const wsp_toke
 	const int len = result->failed ? 0 : result->n_tokens;
 	if( result->n_tokens > 0 && ( !tokens || !times ) ) return fail( WSP_E_POINTER, "tokens/times" );
 	const Context& cx = *c->c;
-	if( cx.windowEnergyBatch < 1 ) return fail( WSP_E_INVALIDARG, "the last wsp_run_chunks_window call ran without token timestamps (or there was none)" );
+	if( cx.windowEnergyBatch < 1 ) return fail( WSP_E_INVALIDARG, "the last window call ran without token timestamps (or there was none)" );
 	if( chunk < 0 || chunk >= cx.windowEnergyBatch ) return fail( WSP_E_BOUNDS, "chunk outside the last window call's batch" );
 	return guarded( [ & ]() -> wsp_status {
 		const Engine& e = *cx.e;
 		auto textOf = [ & ]( int id ) -> const char* { return id >= 0 && id < (int)e.tokenText.size() ? e.tokenText[ (size_t)id ].c_str() : nullptr; };
+		const WindowRow& row = cx.windowRows[ (size_t)chunk ];
 		std::vector<wsp_segment> cut( (size_t)len + 1 );
 		int32_t nCut = 0;
-		WSP_CHECK( windowSegments( textOf, e.tokEot, e.tokBeg, tokens, result, 0, flags, cut.data(), (int32_t)cut.size(), &nCut ) );
+		WSP_CHECK( windowSegments( textOf, e.tokEot, e.tokBeg, tokens, result, row.seek, flags, cut.data(), (int32_t)cut.size(), &nCut ) );
 		// whisper.cpp:3063-3070, 3107-3114: each segment's token times, then its wrapping, in order from the state of a new call
 		std::vector<wsp_token_time> tt( (size_t)len, wsp_token_time{ -1, -1, 0.0f } );
 		std::vector<float> vlen( (size_t)len );
@@ -364,7 +376,7 @@ wsp_status wsp_window_token_times( wsp_context* c, int32_t chunk, const wsp_toke
 			vlen[ (size_t)i ] = voiceLength( t );
 			textLen[ (size_t)i ] = t ? (int)strlen( t ) : 0;
 		}
-		const float* energy = cx.energyHost + (size_t)chunk * cx.energyCap;
+		const float* energy = cx.energyHost + (size_t)row.slot * cx.energyCap;
 		const int nSamples = cx.windowEnergyLen[ (size_t)chunk ];
 		TokenTimeState st;
 		std::vector<wsp_segment> out;
@@ -809,6 +821,7 @@ wsp_status wsp_test_signal_energy( int32_t device, const float* const* pcm, cons
 	{
 		eb.pcm[ b ] = dIn.p + (size_t)b * most;
 		eb.nSamples[ b ] = n_samples[ b ];
+		eb.row[ b ] = (uint8_t)b;
 		if( n_samples[ b ] ) WSP_CUDA( cudaMemcpy( dIn.p + (size_t)b * most, pcm[ b ], (size_t)n_samples[ b ] * 4, cudaMemcpyHostToDevice ) );
 	}
 	WSP_CUDA( kern::signalEnergy( eb, 0 ) );

@@ -234,23 +234,23 @@ namespace wsp
 	static int melFrames( const Context& c, int nSamples ) { return nSamples / ( c.speedUp ? 320 : 160 ); }
 	static const kern::MelTables& melTables( const Context& c ) { return c.speedUp ? c.e->melVocoder : c.e->mel; }
 
-	// log-mel of chunks [0, batch) into slots [slot0, slot0 + batch), in one triple of launches per 16 chunks: pcmOf( b ) /
-	// samplesOf( b ) name chunk b's device PCM
-	template<class P, class N>
-	static int melBatchFromDevicePcm( Context& c, int slot0, int batch, P pcmOf, N samplesOf )
+	// log-mel of chunks [0, batch) into slots slotOf( b ), in one triple of launches per 16 chunks: pcmOf( b ) / samplesOf( b ) name
+	// chunk b's device PCM.  Chunk b's maximum goes to melMax[b], which only this launch reads.
+	template<class S, class P, class N>
+	static int melBatchFromDevicePcm( Context& c, int batch, S slotOf, P pcmOf, N samplesOf )
 	{
 		for( int b0 = 0; b0 < batch; b0 += kern::MEL_BATCH )
 		{
 			kern::MelBatch mb{};
 			mb.count = batch - b0 < kern::MEL_BATCH ? batch - b0 : kern::MEL_BATCH;
-			mb.maxSlots = c.melMax + slot0 + b0;
+			mb.maxSlots = c.melMax + b0;
 			for( int i = 0; i < mb.count; i++ )
 			{
 				const int n = samplesOf( b0 + i );
 				const int nLen = melFrames( c, n );
-				WSP_CHECK( ensureMelSlot( c, slot0 + b0 + i, nLen ) );
+				WSP_CHECK( ensureMelSlot( c, slotOf( b0 + i ), nLen ) );
 				mb.pcm[ i ] = pcmOf( b0 + i );
-				mb.mel[ i ] = c.slots[ slot0 + b0 + i ].mel;
+				mb.mel[ i ] = c.slots[ slotOf( b0 + i ) ].mel;
 				mb.nSamples[ i ] = n;
 				mb.nLen[ i ] = nLen;
 			}
@@ -301,20 +301,21 @@ namespace wsp
 		if( host && !c.energyHost ) WSP_CUDA( cudaHostAlloc( (void**)&c.energyHost, (size_t)c.maxB * c.energyCap * 4, cudaHostAllocDefault ) );
 		return WSP_OK;
 	}
-	// signal energy of chunks [0, batch) into slots [slot0, slot0 + batch) in one launch; pcmOf( b ) / samplesOf( b ) name chunk b's
-	// device PCM.  ensureEnergy has made room.
-	template<class P, class N>
-	static int energyFromDevicePcm( Context& c, int slot0, int batch, P pcmOf, N samplesOf )
+	// signal energy of chunks [0, batch) into slots slotOf( b ) in one launch; pcmOf( b ) / samplesOf( b ) name chunk b's device PCM.
+	// ensureEnergy has made room.
+	template<class S, class P, class N>
+	static int energyFromDevicePcm( Context& c, int batch, S slotOf, P pcmOf, N samplesOf )
 	{
 		kern::EnergyBatch eb{};
-		eb.out = c.energy + (size_t)slot0 * c.energyCap;
+		eb.out = c.energy;
 		eb.stride = (int64_t)c.energyCap;
 		eb.count = batch;
 		for( int b = 0; b < batch; b++ )
 		{
 			eb.pcm[ b ] = pcmOf( b );
 			eb.nSamples[ b ] = samplesOf( b );
-			c.energyLen[ (size_t)( slot0 + b ) ] = eb.nSamples[ b ];
+			eb.row[ b ] = (uint8_t)slotOf( b );
+			c.energyLen[ (size_t)slotOf( b ) ] = eb.nSamples[ b ];
 		}
 		WSP_CUDA( kern::signalEnergy( eb, c.stream ) );
 		launched();
@@ -348,10 +349,11 @@ namespace wsp
 		if( ( !pcmHost && nSamples != 0 ) || nSamples < 0 ) return fail( WSP_E_INVALIDARG, "pcm" );
 		if( c.tokenTimestamps ) WSP_CHECK( ensureEnergy( c, (size_t)( nSamples > 0 ? nSamples : 1 ), false ) );
 		return pcmToMelTimed( c, pcmHost, nSamples, [ & ]() -> int {
+			auto slotOf = [ & ]( int ) { return slot; };
 			auto pcmOf = [ & ]( int ) { return (const float*)c.pcmDev; };
 			auto samplesOf = [ & ]( int ) { return nSamples; };
-			WSP_CHECK( melBatchFromDevicePcm( c, slot, 1, pcmOf, samplesOf ) );
-			return c.tokenTimestamps ? energyFromDevicePcm( c, slot, 1, pcmOf, samplesOf ) : WSP_OK;
+			WSP_CHECK( melBatchFromDevicePcm( c, 1, slotOf, pcmOf, samplesOf ) );
+			return c.tokenTimestamps ? energyFromDevicePcm( c, 1, slotOf, pcmOf, samplesOf ) : WSP_OK;
 		} );
 	}
 
@@ -406,7 +408,8 @@ namespace wsp
 	// ===============================================================================================================
 	// encoder
 	// ===============================================================================================================
-	static int encodeAsync( Context& c, const int32_t* offsets, int batch )
+	// chunk b's window is frames [offsets[b], offsets[b] + 2n) of slot slots[b]'s log-mel (slots == nullptr: slot b; offsets == nullptr: 0)
+	static int encodeAsync( Context& c, const int32_t* slots, const int32_t* offsets, int batch )
 	{
 		Engine& e = *c.e;
 		const HParams& hp = e.hp;
@@ -418,8 +421,9 @@ namespace wsp
 		cudaStream_t s = c.stream;
 		for( int b = 0; b < batch; b++ )
 		{
-			const MelSlot& ms = c.slots[ b ];
-			if( !ms.mel ) return fail( WSP_E_INVALIDARG, "no mel in slot " + std::to_string( b ) );
+			const int slot = slots ? slots[ b ] : b;
+			const MelSlot& ms = c.slots[ slot ];
+			if( !ms.mel ) return fail( WSP_E_INVALIDARG, "no mel in slot " + std::to_string( slot ) );
 			const int off = offsets ? offsets[ b ] : 0;
 			if( off < 0 ) return fail( WSP_E_INVALIDARG, "negative mel offset" );
 			WSP_CUDA( kern::melWindow( ms.mel, ms.nLen, off, c.melF16 + (size_t)b * rowsPad * 80, frames, s ) );
@@ -516,7 +520,7 @@ namespace wsp
 	{
 		if( batch < 1 || batch > c.maxB ) return fail( WSP_E_BOUNDS, "batch exceeds the context's max_batch" );
 		WSP_CUDA( cudaSetDevice( c.e->device ) );
-		return timeStage( c, 1, [ & ]() -> int { return encodeAsync( c, offsets, batch ); } );
+		return timeStage( c, 1, [ & ]() -> int { return encodeAsync( c, nullptr, offsets, batch ); } );
 	}
 
 	// ===============================================================================================================
@@ -887,10 +891,11 @@ namespace wsp
 	constexpr int kEotLag = 8;
 
 	int ctxRunChunks( Context& c, const float* const* pcm, const int32_t* nSamples, int batch, const int32_t* prompt, int nPrompt, int nDecode,
-		int32_t* tokensOut, int32_t* nOut, float* stageMs, bool resident, const WindowOut* window )
+		int32_t* tokensOut, int32_t* nOut, float* stageMs, bool resident, const WindowOut* window, const WindowRow* rows )
 	{
 		const HParams& hp = c.e->hp;
 		if( batch < 1 || batch > c.maxB ) return fail( WSP_E_BOUNDS, "batch exceeds the context's max_batch" );
+		auto slotOf = [ & ]( int b ) { return rows ? rows[ b ].slot : b; };
 		if( !prompt || nPrompt < 1 || nPrompt > kMaxDecodeTokens ) return fail( WSP_E_INVALIDARG, "prompt" );
 		// every id indexes the embedding table, as ctxDecode's tokens do; at most one is the language sentinel
 		int autoPos = -1;
@@ -910,26 +915,44 @@ namespace wsp
 		for( int b = 0; b < batch; b++ )
 		{
 			if( !resident && nSamples[ b ] < 0 ) return fail( WSP_E_INVALIDARG, "n_samples" );
-			if( resident && !c.slots[ b ].pcm ) return fail( WSP_E_INVALIDARG, "no resident PCM in slot " + std::to_string( b ) + " (call wsp_upload_pcm)" );
+			if( resident && !c.slots[ slotOf( b ) ].pcm )
+				return fail( WSP_E_INVALIDARG, "no resident PCM in slot " + std::to_string( slotOf( b ) ) + " (call wsp_upload_pcm)" );
+			// whisper_lang_auto_detect( offset_ms ) refuses an offset at or past the end of the mel (whisper.cpp:2440-2443)
+			if( rows && detect && rows[ b ].seek >= melFrames( c, c.slots[ rows[ b ].slot ].pcmSamples ) )
+				return fail( WSP_E_INVALIDARG, "WSP_TOKEN_LANGUAGE_AUTO with a span offset at or past the end of its source" );
 		}
 		const bool untilEot = nOut != nullptr;
 		if( window && window->cap < nDecode ) return fail( WSP_E_BOUNDS, "cap is below n_max" );
-		// each window runs at seek 0 over its chunk's mel length (whisper.cpp:2810-2818); one of at most 100 frames runs none (:2871)
-		std::vector<int32_t> seekEnd( window ? (size_t)batch : 0 );
-		for( size_t b = 0; b < seekEnd.size(); b++ ) seekEnd[ b ] = melFrames( c, resident ? c.slots[ b ].pcmSamples : nSamples[ b ] );
+		// each window runs from its seek to its seek_end (whisper.cpp:2810-2818): seek 0 and the chunk's mel length, or a row's span; one
+		// of at most 100 frames runs none (:2816, 2871).  The window rule reads the two only as seek_end - seek.
+		std::vector<int32_t> toEnd( window ? (size_t)batch : 0 );
+		for( size_t b = 0; b < toEnd.size(); b++ )
+			toEnd[ b ] = rows ? rows[ b ].seekEnd - rows[ b ].seek : melFrames( c, resident ? c.slots[ b ].pcmSamples : nSamples[ b ] );
+		// the slots whose log-mel (and energy) the call computes: each chunk's own, or each source slot of the rows once
+		std::vector<int> srcs;
+		if( rows )
+		{
+			std::vector<char> named( (size_t)c.maxB, 0 );
+			for( int b = 0; b < batch; b++ )
+				if( !named[ (size_t)rows[ b ].slot ] ) { named[ (size_t)rows[ b ].slot ] = 1; srcs.push_back( rows[ b ].slot ); }
+		}
+		else
+			for( int b = 0; b < batch; b++ ) srcs.push_back( b );
+		const int nSrc = (int)srcs.size();
+		auto srcSlot = [ & ]( int i ) { return srcs[ (size_t)i ]; };
 		c.lastLangIds.clear();
 		c.lastLangProbs.clear();
 		WSP_CUDA( cudaSetDevice( c.e->device ) );
-		// a window call with token timestamps on computes every chunk's signal energy right after the log-mel
+		// a window call with token timestamps on computes every source's signal energy right after the log-mel
 		const bool energy = window && c.tokenTimestamps;
 		if( window ) c.windowEnergyBatch = 0;
-		std::vector<int> energyLen( energy ? (size_t)batch : 0 );
+		std::vector<int> energyLen( energy ? (size_t)batch : 0 );   // of each chunk's source
 		if( energy )
 		{
 			size_t most = 1;
 			for( int b = 0; b < batch; b++ )
 			{
-				energyLen[ (size_t)b ] = resident ? c.slots[ b ].pcmSamples : nSamples[ b ];
+				energyLen[ (size_t)b ] = resident ? c.slots[ slotOf( b ) ].pcmSamples : nSamples[ b ];
 				most = std::max( most, (size_t)energyLen[ (size_t)b ] );
 			}
 			WSP_CHECK( ensureEnergy( c, most, true ) );
@@ -939,10 +962,10 @@ namespace wsp
 		if( resident )
 		{
 			// inputs already in HBM (wsp_upload_pcm): the log-mel front end still runs inside the timed region
-			auto pcmOf = [ & ]( int b ) { return (const float*)c.slots[ b ].pcm; };
-			auto samplesOf = [ & ]( int b ) { return c.slots[ b ].pcmSamples; };
-			WSP_CHECK( melBatchFromDevicePcm( c, 0, batch, pcmOf, samplesOf ) );
-			if( energy ) WSP_CHECK( energyFromDevicePcm( c, 0, batch, pcmOf, samplesOf ) );
+			auto pcmOf = [ & ]( int i ) { return (const float*)c.slots[ srcSlot( i ) ].pcm; };
+			auto samplesOf = [ & ]( int i ) { return c.slots[ srcSlot( i ) ].pcmSamples; };
+			WSP_CHECK( melBatchFromDevicePcm( c, nSrc, srcSlot, pcmOf, samplesOf ) );
+			if( energy ) WSP_CHECK( energyFromDevicePcm( c, nSrc, srcSlot, pcmOf, samplesOf ) );
 		}
 		else
 		{
@@ -960,11 +983,13 @@ namespace wsp
 			}
 			auto pcmOf = [ & ]( int b ) { return (const float*)( c.pcmDev + offs[ (size_t)b ] ); };
 			auto samplesOf = [ & ]( int b ) { return (int)nSamples[ b ]; };
-			WSP_CHECK( melBatchFromDevicePcm( c, 0, batch, pcmOf, samplesOf ) );
-			if( energy ) WSP_CHECK( energyFromDevicePcm( c, 0, batch, pcmOf, samplesOf ) );
+			WSP_CHECK( melBatchFromDevicePcm( c, batch, srcSlot, pcmOf, samplesOf ) );
+			if( energy ) WSP_CHECK( energyFromDevicePcm( c, batch, srcSlot, pcmOf, samplesOf ) );
 		}
 		WSP_CUDA( cudaEventRecord( c.ev[ 1 ], s ) );
-		WSP_CHECK( encodeAsync( c, nullptr, batch ) );
+		std::vector<int32_t> rowSlot( rows ? (size_t)batch : 0 ), rowSeek( rows ? (size_t)batch : 0 );
+		for( size_t b = 0; b < rowSlot.size(); b++ ) { rowSlot[ b ] = rows[ b ].slot; rowSeek[ b ] = rows[ b ].seek; }
+		WSP_CHECK( encodeAsync( c, rows ? rowSlot.data() : nullptr, rows ? rowSeek.data() : nullptr, batch ) );
 		WSP_CUDA( cudaEventRecord( c.ev[ 2 ], s ) );
 		// prompt step: same prompt for every chunk, first sample uses the initial-timestamp rules (whisper.cpp:2943); with the
 		// language sentinel the tokens uploaded are the detection pass's [sot] per chunk, and langPick writes the prompts
@@ -1006,8 +1031,8 @@ namespace wsp
 				int preEnded = 0;
 				for( int b = 0; b < batch; b++ )
 				{
-					ctl[ 4 + (size_t)b ] = seekEnd[ (size_t)b ];
-					if( seekEnd[ (size_t)b ] > 100 ) continue;
+					ctl[ 4 + (size_t)b ] = toEnd[ (size_t)b ];
+					if( toEnd[ (size_t)b ] > 100 ) continue;
 					st[ (size_t)b ] = wsp::WindowState{ 0, 0, 0, 0, 1 };
 					ends[ (size_t)b ] = -1;
 					preEnded++;
@@ -1046,9 +1071,11 @@ namespace wsp
 			WSP_CUDA( cudaMemcpyAsync( winSt.data(), c.winState, winSt.size() * sizeof( wsp::WindowState ), cudaMemcpyDeviceToHost, s ) );
 			WSP_CUDA( cudaMemcpyAsync( tdLog.data(), c.tokenLog, tdLog.size() * sizeof( kern::TokenData ), cudaMemcpyDeviceToHost, s ) );
 		}
-		for( size_t b = 0; b < energyLen.size(); b++ )
-			if( energyLen[ b ] > 0 )
-				WSP_CUDA( cudaMemcpyAsync( c.energyHost + b * c.energyCap, c.energy + b * c.energyCap, (size_t)energyLen[ b ] * 4, cudaMemcpyDeviceToHost, s ) );
+		if( energy )
+			for( const int slot : srcs )
+				if( c.energyLen[ (size_t)slot ] > 0 )
+					WSP_CUDA( cudaMemcpyAsync( c.energyHost + (size_t)slot * c.energyCap, c.energy + (size_t)slot * c.energyCap,
+						(size_t)c.energyLen[ (size_t)slot ] * 4, cudaMemcpyDeviceToHost, s ) );
 		std::vector<int32_t> langIds( detect ? (size_t)batch : 0 );
 		std::vector<float> langProbs( detect ? (size_t)batch * c.e->nLangs : 0 );
 		if( detect )
@@ -1063,6 +1090,8 @@ namespace wsp
 		{
 			c.windowEnergyBatch = batch;
 			c.windowEnergyLen.swap( energyLen );
+			c.windowRows.resize( (size_t)batch );
+			for( int b = 0; b < batch; b++ ) c.windowRows[ (size_t)b ] = rows ? rows[ b ] : WindowRow{ b, 0, toEnd[ (size_t)b ] };
 		}
 		if( window )
 			for( int b = 0; b < batch; b++ )
@@ -1089,5 +1118,26 @@ namespace wsp
 		const float m2 = addStage( c, 2, c.ev[ 2 ], c.ev[ 3 ], steps );
 		if( stageMs ) { stageMs[ 0 ] = m0; stageMs[ 1 ] = m1; stageMs[ 2 ] = m2; }
 		return WSP_OK;
+	}
+
+	// whisper_full( clip of spans[b].slot, offset_ms, duration_ms )'s window bounds (whisper.cpp:2810-2811) for every row, then the
+	// window call over them.  The seek arithmetic cannot overflow: offset_ms / 10, |duration_ms| / 10 and n_len = n_samples / 160 are
+	// each below 2^31 / 10, so seek_end stays within int32.
+	int ctxRunSpans( Context& c, const wsp_window_span* spans, int batch, const int32_t* prompt, int nPrompt, int nDecode, float* stageMs,
+		const WindowOut& window )
+	{
+		if( batch < 1 || batch > c.maxB ) return fail( WSP_E_BOUNDS, "batch exceeds the context's max_batch" );
+		std::vector<WindowRow> rows( (size_t)batch );
+		for( int b = 0; b < batch; b++ )
+		{
+			const wsp_window_span& sp = spans[ b ];
+			if( sp.slot < 0 || sp.slot >= c.maxB ) return fail( WSP_E_BOUNDS, "span slot outside max_batch" );
+			if( !c.slots[ sp.slot ].pcm ) return fail( WSP_E_INVALIDARG, "no resident PCM in slot " + std::to_string( sp.slot ) + " (call wsp_upload_pcm)" );
+			if( sp.offset_ms < 0 ) return fail( WSP_E_INVALIDARG, "negative offset_ms" );
+			const int nLen = melFrames( c, c.slots[ sp.slot ].pcmSamples );
+			const int seek = sp.offset_ms / 10;
+			rows[ (size_t)b ] = WindowRow{ sp.slot, seek, seek + ( sp.duration_ms == 0 ? nLen : sp.duration_ms / 10 ) };
+		}
+		return ctxRunChunks( c, nullptr, nullptr, batch, prompt, nPrompt, nDecode, nullptr, nullptr, stageMs, true, &window, rows.data() );
 	}
 }

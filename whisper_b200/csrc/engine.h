@@ -102,6 +102,12 @@ namespace wsp
 		int stereoFrames = 0;      // 0: the slot has no stereo (wsp_upload_pcm drops it)
 	};
 
+	// one row of a window call: the slot whose log-mel it encodes and whisper_full's seek_start / seek_end, in mel frames
+	struct WindowRow
+	{
+		int slot, seek, seekEnd;
+	};
+
 	// per-kernel-kind device time of the decoder, collected by an instrumented (un-graphed) pass: wsp_profile_decode
 	enum KernelKind { KK_SKINNY = 0, KK_CROSS = 1, KK_SELF = 2, KK_OTHER = 3, KK_COUNT = 4 };
 	struct KernelProfile
@@ -131,7 +137,7 @@ namespace wsp
 		int maxB = 0;
 		cudaStream_t stream = nullptr;
 		std::vector<MelSlot> slots;
-		int* melMax = nullptr;          // [maxB] ordered-int maxima
+		int* melMax = nullptr;          // [maxB] ordered-int maxima of one mel launch's chunks
 		float* pcmDev = nullptr; size_t pcmCap = 0;
 		uint64_t devBytes = 0;          // device memory this context holds (timingsPrint's memory table)
 		bool speedUp = false;           // whole-clip log-mels through the 2x phase vocoder (wsp_set_speed_up)
@@ -178,8 +184,8 @@ namespace wsp
 		int* nEndedHost = nullptr;      // mapped pinned copy of nEnded, written by the last kernel of every step
 		int* nEndedMapped = nullptr;    // its device address
 		cudaEvent_t blockEv[ 2 ] = { nullptr, nullptr };   // ends of the last two enqueued step blocks
-		// whisper_full's window rule of wsp_run_chunks_window, passed to the armed sampler of both calls; winCtl[0] = 0 (EOT) or 1 (rule)
-		int* winCtl = nullptr;          // [4 + maxB] on | max_tokens | single_segment | n_max, then each row's seek_end
+		// whisper_full's window rule of the window calls, passed to the armed sampler of both calls; winCtl[0] = 0 (EOT) or 1 (rule)
+		int* winCtl = nullptr;          // [4 + maxB] on | max_tokens | single_segment | n_max, then each row's seek_end - seek
 		wsp::WindowState* winState = nullptr;   // [maxB]
 		kern::TokenData* tokenLog = nullptr;    // [maxB][histCap] every armed step's TokenData
 		// per-chunk language detection of a run_chunks* call whose prompt holds WSP_TOKEN_LANGUAGE_AUTO (lang_pick_kernel)
@@ -193,8 +199,9 @@ namespace wsp
 		float* energyHost = nullptr;    // [maxB][energyCap] pinned: the last window call's energy, copied back with its tokens
 		size_t energyCap = 0;
 		std::vector<int> energyLen;     // [maxB] samples of each slot's device energy
-		int windowEnergyBatch = 0;      // batch of the last wsp_run_chunks_window call if it computed the energy, else 0
-		std::vector<int> windowEnergyLen;   // [that batch] samples of each chunk's energy in energyHost
+		int windowEnergyBatch = 0;      // batch of the last window call if it computed the energy, else 0
+		std::vector<int> windowEnergyLen;   // [that batch] samples of each chunk's source energy in energyHost
+		std::vector<WindowRow> windowRows;  // [that batch] each chunk's source slot (its energy's row in energyHost) and seek
 		// wsp_chunk_speakers: the segments' jobs, then their answers, in one device buffer
 		uint8_t* speakerBuf = nullptr;
 		size_t speakerCap = 0;          // segments it holds
@@ -264,7 +271,11 @@ namespace wsp
 		wsp_window_result* results;     // [batch]
 	};
 	// nOut == nullptr and window == nullptr: nDecode steps for every chunk (wsp_run_chunks*); nOut: each chunk ends at its first EOT
-	// (wsp_run_chunks_until_eot); window: each chunk ends by whisper_full's window rule, nDecode = n_max (wsp_run_chunks_window)
+	// (wsp_run_chunks_until_eot); window: each chunk ends by whisper_full's window rule, nDecode = n_max (wsp_run_chunks_window).
+	// rows (window calls from resident PCM only): chunk b is rows[b]'s window, else chunk b is slot b's at seek 0 over its mel length.
 	int ctxRunChunks( Context& c, const float* const* pcm, const int32_t* nSamples, int batch, const int32_t* prompt, int nPrompt, int nDecode,
-		int32_t* tokensOut, int32_t* nOut, float* stageMs, bool resident, const WindowOut* window = nullptr );
+		int32_t* tokensOut, int32_t* nOut, float* stageMs, bool resident, const WindowOut* window = nullptr, const WindowRow* rows = nullptr );
+	// wsp_run_spans_window
+	int ctxRunSpans( Context& c, const wsp_window_span* spans, int batch, const int32_t* prompt, int nPrompt, int nDecode, float* stageMs,
+		const WindowOut& window );
 }

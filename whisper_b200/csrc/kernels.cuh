@@ -60,7 +60,7 @@ namespace kern
 	cudaError_t melWindow( const float* mel, int nLen, int offset, __half* dst, int frames, cudaStream_t s );
 
 	// ---- signal energy of token-level timestamps (get_signal_energy, whisper.cpp:3356-3372) ----------------------------------
-	// every chunk of a batch in one launch: chunk b's pcm[b][nSamples[b]] -> out[b * stride + i] = (sum over j = -32..32 with
+	// every chunk of a batch in one launch: chunk b's pcm[b][nSamples[b]] -> out[row[b] * stride + i] = (sum over j = -32..32 with
 	// 0 <= i + j < n of |x[i + j]|) / 65, the sum in f32 in that order of j, so the result is bit-identical to the reference's
 	constexpr int ENERGY_BATCH = 256;
 	constexpr int ENERGY_HW = 32;
@@ -68,7 +68,8 @@ namespace kern
 	{
 		const float* pcm[ ENERGY_BATCH ];
 		int nSamples[ ENERGY_BATCH ];
-		float* out;                    // [count][stride]
+		uint8_t row[ ENERGY_BATCH ];   // the output row of chunk b (a context slot, < 256)
+		float* out;                    // [rows][stride]
 		int64_t stride;
 		int count;
 	};
@@ -164,8 +165,8 @@ namespace kern
 		volatile int* nEndedHost = nullptr;
 		// armed callers also pass these (wsp_run_chunks_window): the step's TokenData goes to tokenLog[b][*dStep], and while
 		// winCtl[0] is set a row ends by whisper_full's window rule (window_rule.h) instead of at its first EOT.  winCtl = { on,
-		// max_tokens, single_segment, n_max }, then seekEnd[B]; winState[B] is the rows' state, and a row whose endStep the caller
-		// set non-zero never runs the rule
+		// max_tokens, single_segment, n_max }, then seek_end - seek of each row [B] (the rule runs at seek 0 over it, which decides
+		// as at seek over seek_end); winState[B] is the rows' state, and a row whose endStep the caller set non-zero never runs the rule
 		const int* winCtl = nullptr;
 		wsp::WindowState* winState = nullptr;
 		TokenData* tokenLog = nullptr;

@@ -248,7 +248,7 @@ namespace kern
 		float sum = 0.0f;
 #pragma unroll
 		for( int j = 0; j <= 2 * ENERGY_HW; j++ ) sum += sx[ threadIdx.x + j ];
-		eb.out[ b * eb.stride + i ] = sum / (float)( 2 * ENERGY_HW + 1 );
+		eb.out[ eb.row[ b ] * eb.stride + i ] = sum / (float)( 2 * ENERGY_HW + 1 );
 	}
 	cudaError_t signalEnergy( const EnergyBatch& eb, cudaStream_t s )
 	{

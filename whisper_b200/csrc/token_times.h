@@ -32,7 +32,8 @@ namespace wsp
 		return res;
 	}
 
-	inline int timestampToSample( int64_t t, int nSamples ) { return std::max( 0, std::min( nSamples - 1, (int)( ( t * 16000 ) / 100 ) ) ); }   // :3320-3322
+	// :3320-3322, clamped before the narrowing so that a span's times past 2^31 samples (offsets beyond 37 h) clamp as well
+	inline int timestampToSample( int64_t t, int nSamples ) { return (int)std::max<int64_t>( 0, std::min<int64_t>( nSamples - 1, ( t * 16000 ) / 100 ) ); }
 	inline int64_t sampleToTimestamp( int iSample ) { return ( 100 * (int64_t)iSample ) / 16000; }   // :3324-3326
 
 	// whisper_exp_compute_token_level_timestamps (whisper.cpp:3374-3600) for one segment of n tokens over [t0, t1] (10 ms units):
