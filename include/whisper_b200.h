@@ -400,13 +400,24 @@ wsp_status wsp_profile_decode( wsp_context* c, int32_t batch, int32_t n_steps, f
  *   "enc.h"                [n][4d]      f16 MLP hidden gelu(LN2(x) W1^T + b1) of the last encoded layer
  *   "cross_k", "cross_v"   [L][H][n][64] f16 cross-attention memories (K scaled by 64^-0.25)
  *   "self_k", "self_v"     [L][H][n_text_ctx][64] f16 decoder self-KV cache (K scaled by 64^-0.25); row j = text position j
- *   "dec.x"                [8][d]       f32 decoder residual stream (shared by all slots)
+ * The decoder tensors are the rows of chunk `slot` in the last decoder pass that ran kernel by kernel (every pass while a decoder stop
+ * is set; N = that pass's tokens per chunk, d = n_text_state):
+ *   "dec.x"                [N][d]       f32 residual stream
+ *   "dec.q"                [N][d]       f32 query of the last self or cross attention (scaled by 64^-0.25)
+ *   "dec.attn"             [N][d]       f16 output of the last self or cross attention (head h in columns [64h, 64h + 64))
+ *   "dec.h"                [N][4d]      f16 MLP hidden gelu(LN3(x) W1^T + b1)
  *   "energy"               [n_samples]  f32 signal energy of the chunk's PCM (wsp_set_token_timestamps); empty before any
  *   "pcm"                  [n_samples]  f32 the slot's resident mono PCM (wsp_upload_pcm, or the downmix of wsp_upload_pcm_stereo)
  *   "pcm_stereo"           [n_frames][2] f32 the slot's stereo pairs (wsp_upload_pcm_stereo); empty after wsp_upload_pcm */
 wsp_status wsp_get_tensor( wsp_context* c, const char* name, int32_t slot, float* dst, size_t cap_floats, size_t* n_floats );
 /* debug: run only the first n encoder layers (negative = all) */
 wsp_status wsp_debug_set_encoder_layers( wsp_context* c, int32_t n );
+/* debug: end every decoder pass after op `op` of decoder layer `layer` (0 LN + QKV with the self-KV append, 1 self attention, 2 self
+ * out-projection + residual, 3 LN + cross Q, 4 cross attention, 5 cross out-projection + residual, 6 LN + fc1 + GELU, 7 fc2 + residual);
+ * layer -1 ends it after the embedding.  While a stop is set every wsp_decode runs kernel by kernel whatever its n_tokens and the step
+ * mode, without the CUDA graph, the final LayerNorm, the logits or the probabilities, and a call that would sample fails with
+ * WSP_E_INVALIDARG.  (-1, -1) clears the stop. */
+wsp_status wsp_debug_set_decoder_stop( wsp_context* c, int32_t layer, int32_t op );
 /* The CPU reference accumulates the decoder's V^T*P product in f16, per thread (Whisper/source/ggml.c:4680-4722), so its logits
  * depend on its thread count.  n = the cpuThreads the reference would be run with (sFullParams::cpuThreads; default 4 =
  * whisper_full_default_params, Whisper/source/whisper.cpp:2605); the decoder reproduces that arithmetic for n = 1..16 in every
@@ -455,6 +466,8 @@ wsp_status wsp_test_speakers( const float* lr, int32_t n_frames, const wsp_segme
  * mean time of one launch over `iters` more launches between CUDA events */
 wsp_status wsp_test_signal_energy( int32_t device, const float* const* pcm, const int32_t* n_samples, int32_t batch, float* const* energy,
 	int32_t iters, float* ms );
+/* the all-logits vocabulary softmax alone: rows of n logits -> probs with the reference's f16-table exp (host pointers) */
+wsp_status wsp_test_softmax_rows( int32_t device, int32_t rows, int32_t n, const float* logits, float* probs );
 /* LayerNorm rows x d f32 -> f16 bit patterns */
 wsp_status wsp_test_layernorm( int32_t device, int32_t rows, int32_t d, const float* x, const float* gamma, const float* beta, uint16_t* out );
 

@@ -74,10 +74,10 @@ EXPORTS = [
     "wsp_engine_create", "wsp_engine_create_from_image", "wsp_engine_destroy", "wsp_engine_weight_bytes",
     "wsp_context_create", "wsp_context_destroy", "wsp_synchronize",
     "wsp_context_device_bytes", "wsp_pcm_to_mel", "wsp_pcm_to_mel_window", "wsp_set_mel", "wsp_mel_len", "wsp_get_mel", "wsp_encode", "wsp_set_audio_ctx", "wsp_set_speed_up", "wsp_decode", "wsp_get_logits", "wsp_get_probs",
-    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_run_chunks_until_eot", "wsp_get_chunk_languages", "wsp_run_chunks_window", "wsp_run_spans_window", "wsp_window_segments", "wsp_set_token_timestamps", "wsp_window_token_times", "wsp_upload_pcm", "wsp_upload_pcm_stereo", "wsp_chunk_speakers", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
+    "wsp_detect_language", "wsp_run_chunks", "wsp_run_chunks_resident", "wsp_run_chunks_until_eot", "wsp_get_chunk_languages", "wsp_run_chunks_window", "wsp_run_spans_window", "wsp_window_segments", "wsp_set_token_timestamps", "wsp_window_token_times", "wsp_upload_pcm", "wsp_upload_pcm_stereo", "wsp_chunk_speakers", "wsp_timer_start", "wsp_timer_stop", "wsp_profile_decode", "wsp_get_tensor", "wsp_debug_set_encoder_layers", "wsp_debug_set_decoder_stop", "wsp_debug_set_graph", "wsp_debug_set_step_mode", "wsp_debug_enable_step_timing", "wsp_debug_step_timing", "wsp_set_reference_threads",
     "wsp_host_alloc", "wsp_host_free", "wsp_timings",
     "wsp_replicas_create", "wsp_replicas_count", "wsp_replicas_run_chunks", "wsp_replicas_debug_fail_next", "wsp_replicas_destroy",
-    "wsp_test_gemm", "wsp_test_attention", "wsp_test_skinny", "wsp_test_layernorm", "wsp_test_sample", "wsp_test_window_rule", "wsp_test_token_times", "wsp_test_signal_energy",
+    "wsp_test_gemm", "wsp_test_attention", "wsp_test_skinny", "wsp_test_layernorm", "wsp_test_sample", "wsp_test_softmax_rows", "wsp_test_window_rule", "wsp_test_token_times", "wsp_test_signal_energy",
     "wsp_test_speakers",
 ]
 
@@ -163,6 +163,7 @@ def lib():
     sig("wsp_profile_decode", i32, [vp, i32, i32, fp, ip])
     sig("wsp_get_tensor", i32, [vp, C.c_char_p, i32, fp, sz, C.POINTER(sz)])
     sig("wsp_debug_set_encoder_layers", i32, [vp, i32])
+    sig("wsp_debug_set_decoder_stop", i32, [vp, i32, i32])
     sig("wsp_debug_set_graph", i32, [vp, i32])
     sig("wsp_set_reference_threads", i32, [vp, i32])
     sig("wsp_debug_set_step_mode", i32, [vp, i32])
@@ -178,6 +179,7 @@ def lib():
     sig("wsp_replicas_debug_fail_next", i32, [vp, i32])
     sig("wsp_replicas_destroy", None, [vp])
     sig("wsp_test_sample", i32, [i32, i32, i32, fp, ip, i32, i32, fp, C.POINTER(TokenData)])
+    sig("wsp_test_softmax_rows", i32, [i32, i32, i32, fp, fp])
     sig("wsp_test_gemm", i32, [i32, i32, i32, i32, u16p, u16p, fp, i32, i32, fp])
     sig("wsp_test_attention", i32, [i32, i32, i32, u16p, u16p, u16p, fp, i32, fp])
     sig("wsp_test_skinny", i32, [i32, i32, i32, i32, u16p, u16p, fp, i32, fp])
@@ -603,6 +605,12 @@ class Context:
     def set_encoder_layers(self, n: int):
         check(self.L.wsp_debug_set_encoder_layers(self.h, n))
 
+    def set_decoder_stop(self, layer: int, op: int):
+        """End every decoder pass after op `op` (0 QKV, 1 self attention, 2 self-out, 3 cross Q, 4 cross attention, 5 cross-out,
+        6 fc1, 7 fc2) of layer `layer`; layer -1 = after the embedding, (-1, -1) = no stop.  Stopped passes run kernel by kernel and
+        must not sample (DECODE_NO_SAMPLE or DECODE_ALL_LOGITS)."""
+        check(self.L.wsp_debug_set_decoder_stop(self.h, int(layer), int(op)))
+
     def set_reference_threads(self, n: int):
         check(self.L.wsp_set_reference_threads(self.h, n))
 
@@ -735,6 +743,15 @@ def test_sample(logits: np.ndarray, special4, force_timestamp=False, is_initial=
     sp = np.ascontiguousarray(special4, np.int32)
     check(lib().wsp_test_sample(device, rows, nv, _f(lg), _i(sp), int(force_timestamp), int(is_initial), _f(probs), out))
     return probs, [dict(id=t.id, tid=t.tid, p=t.p, pt=t.pt, ptsum=t.ptsum) for t in out]
+
+
+def test_softmax_rows(logits: np.ndarray, device: int = 0):
+    """rows of logits -> probs [rows][n] from softmaxRows alone (the all-logits vocabulary softmax)"""
+    lg = np.ascontiguousarray(logits, np.float32)
+    rows, n = lg.shape
+    probs = np.empty_like(lg)
+    check(lib().wsp_test_softmax_rows(device, rows, n, _f(lg), _f(probs)))
+    return probs
 
 
 class Replicas:

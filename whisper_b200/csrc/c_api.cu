@@ -507,7 +507,15 @@ wsp_status wsp_get_tensor( wsp_context* cc, const char* name, int32_t slot, floa
 		}
 		return WSP_OK;
 	}
-	else if( nm == "dec.x" ) { f32 = c.xd; n = (size_t)d * 8; }
+	else if( nm == "dec.x" || nm == "dec.q" || nm == "dec.attn" || nm == "dec.h" )
+	{
+		// rows [slot * N, slot * N + N) of the last kernel-by-kernel decoder pass, N tokens per chunk
+		const size_t dt = (size_t)hp.n_text_state, N = (size_t)c.lastPerOpN;
+		if( nm == "dec.x" ) { f32 = c.xd + (size_t)slot * N * dt; n = N * dt; }
+		else if( nm == "dec.q" ) { f32 = c.qd + (size_t)slot * N * dt; n = N * dt; }
+		else if( nm == "dec.attn" ) { f16 = c.attnD + (size_t)slot * N * dt; n = N * dt; }
+		else { f16 = c.hD + (size_t)slot * N * 4 * dt; n = N * 4 * dt; }
+	}
 	else if( nm == "energy" ) { f32 = c.energy + (size_t)slot * c.energyCap; n = (size_t)c.energyLen[ (size_t)slot ]; }
 	else if( nm == "pcm" ) { f32 = c.slots[ slot ].pcm; n = (size_t)c.slots[ slot ].pcmSamples; }
 	else if( nm == "pcm_stereo" ) { f32 = c.slots[ slot ].stereo; n = (size_t)2 * c.slots[ slot ].stereoFrames; }
@@ -567,6 +575,16 @@ wsp_status wsp_debug_set_encoder_layers( wsp_context* c, int32_t n )
 {
 	if( !c ) return fail( WSP_E_POINTER, "context" );
 	c->c->debugEncLayers = n;
+	return WSP_OK;
+}
+wsp_status wsp_debug_set_decoder_stop( wsp_context* c, int32_t layer, int32_t op )
+{
+	if( !c ) return fail( WSP_E_POINTER, "context" );
+	const bool clear = layer == -1 && op == -1;
+	if( !clear && ( layer < -1 || layer >= c->c->e->hp.n_text_layer || op < 0 || op > 7 ) )
+		return fail( WSP_E_INVALIDARG, "decoder stop: layer in [-1, n_text_layer), op in [0, 7], or (-1, -1)" );
+	c->c->debugDecLayer = layer;
+	c->c->debugDecOp = op;
 	return WSP_OK;
 }
 wsp_status wsp_set_reference_threads( wsp_context* c, int32_t n )
@@ -888,6 +906,22 @@ wsp_status wsp_test_sample( int32_t device, int32_t rows, int32_t n_vocab, const
 	g_launchCount.fetch_add( 2 );
 	WSP_CUDA( cudaMemcpy( out, dout.p, (size_t)rows * sizeof( wsp_token_data ), cudaMemcpyDeviceToHost ) );
 	if( probs ) WSP_CUDA( cudaMemcpy( probs, dp.p, (size_t)rows * n_vocab * 4, cudaMemcpyDeviceToHost ) );
+	return WSP_OK;
+}
+
+// the all-logits vocabulary softmax alone (softmaxRows, the kernel behind wsp_get_probs after WSP_DECODE_ALL_LOGITS)
+wsp_status wsp_test_softmax_rows( int32_t device, int32_t rows, int32_t n, const float* logits, float* probs )
+{
+	if( !logits || !probs ) return fail( WSP_E_POINTER, "logits/probs" );
+	if( rows < 1 || rows > 4096 || n < 1 ) return fail( WSP_E_INVALIDARG, "rows / n" );
+	WSP_CHECK( requireSm90( device ) );
+	DevTmp<float> dl, dp;
+	WSP_CUDA( dl.alloc( (size_t)rows * n ) ); WSP_CUDA( dp.alloc( (size_t)rows * n ) );
+	WSP_CUDA( cudaMemcpy( dl.p, logits, (size_t)rows * n * 4, cudaMemcpyHostToDevice ) );
+	WSP_CUDA( kern::softmaxRows( dl.p, dp.p, rows, n, 0 ) );
+	WSP_CUDA( cudaDeviceSynchronize() );
+	g_launchCount.fetch_add( 1 );
+	WSP_CUDA( cudaMemcpy( probs, dp.p, (size_t)rows * n * 4, cudaMemcpyDeviceToHost ) );
 	return WSP_OK;
 }
 

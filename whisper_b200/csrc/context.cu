@@ -593,7 +593,12 @@ namespace wsp
 			a.ld = epi == kern::SK_QKV ? d : nOut;
 			return a;
 		};
+		c.lastPerOpN = N;
+		// wsp_debug_set_decoder_stop: the pass ends after op `op` of layer `il` (0 QKV, 1 self attention, 2 self-out, 3 cross Q,
+		// 4 cross attention, 5 cross-out, 6 fc1, 7 fc2)
+		auto stopAfter = [ & ]( int il, int op ) { return c.decoderStopped() && c.debugDecLayer == il && ( il < 0 || c.debugDecOp == op ); };
 		WSP_KERNEL( KK_OTHER, kern::embedTokens( e.tokEmb, e.decPos, c.tokensDev, c.dNPast, c.xd, batch, N, d, s ) ); n++;
+		if( stopAfter( -1, 0 ) ) return WSP_OK;
 		for( int il = 0; il < hp.n_text_layer; il++ )
 		{
 			const DecLayerW& W = e.dec[ il ];
@@ -602,19 +607,27 @@ namespace wsp
 			// LN + (Q | K | V); K, V appended to the f16 self-KV cache in the epilogue (a14)
 			kern::SkinnyArgs a = skinny( W.wqkv, W.bqkv, 3 * d, d, &W.ln1, nullptr, kern::SK_QKV, c.qd );
 			a.kCache = kc; a.vCache = vc; a.d = d; a.N = N; a.nTextCtx = nCtx; a.dNPast = c.dNPast;
-			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( a, s ) );
-			WSP_KERNEL( KK_SELF, kern::selfAttnDecode( c.qd, kc, vc, c.attnD, batch, N, H, d, nCtx, c.dNPast, c.refThreads, s ) );
-			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.wo, W.bo, d, d, nullptr, c.attnD, kern::SK_BIAS_RESID, c.xd ), s ) );
+			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( a, s ) ); n++;
+			if( stopAfter( il, 0 ) ) return WSP_OK;
+			WSP_KERNEL( KK_SELF, kern::selfAttnDecode( c.qd, kc, vc, c.attnD, batch, N, H, d, nCtx, c.dNPast, c.refThreads, s ) ); n++;
+			if( stopAfter( il, 1 ) ) return WSP_OK;
+			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.wo, W.bo, d, d, nullptr, c.attnD, kern::SK_BIAS_RESID, c.xd ), s ) ); n++;
+			if( stopAfter( il, 2 ) ) return WSP_OK;
 			// cross attention (a15)
-			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.wcq, W.bcq, d, d, &W.lnc, nullptr, kern::SK_Q_SCALE, c.qd ), s ) );
+			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.wcq, W.bcq, d, d, &W.lnc, nullptr, kern::SK_Q_SCALE, c.qd ), s ) ); n++;
+			if( stopAfter( il, 3 ) ) return WSP_OK;
 			const size_t crossOff = (size_t)il * c.maxB * hp.n_audio_ctx * d;   // layer stride of the pointer tables, whatever T is
-			WSP_KERNEL( KK_CROSS, kern::crossAttnDecode( c.qd, c.crossK + crossOff, c.crossV + crossOff, c.attnD, batch, N, H, d, T, c.refThreads, s ) );
-			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.wco, W.bco, d, d, nullptr, c.attnD, kern::SK_BIAS_RESID, c.xd ), s ) );
+			WSP_KERNEL( KK_CROSS, kern::crossAttnDecode( c.qd, c.crossK + crossOff, c.crossV + crossOff, c.attnD, batch, N, H, d, T, c.refThreads, s ) ); n++;
+			if( stopAfter( il, 4 ) ) return WSP_OK;
+			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.wco, W.bco, d, d, nullptr, c.attnD, kern::SK_BIAS_RESID, c.xd ), s ) ); n++;
+			if( stopAfter( il, 5 ) ) return WSP_OK;
 			// MLP (a16)
-			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.w1, W.b1, 4 * d, d, &W.ln3, nullptr, kern::SK_GELU_F16, nullptr, c.hD ), s ) );
-			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.w2, W.b2, d, 4 * d, nullptr, c.hD, kern::SK_BIAS_RESID, c.xd ), s ) );
-			n += 8;
+			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.w1, W.b1, 4 * d, d, &W.ln3, nullptr, kern::SK_GELU_F16, nullptr, c.hD ), s ) ); n++;
+			if( stopAfter( il, 6 ) ) return WSP_OK;
+			WSP_KERNEL( KK_SKINNY, kern::skinnyGemm( skinny( W.w2, W.b2, d, 4 * d, nullptr, c.hD, kern::SK_BIAS_RESID, c.xd ), s ) ); n++;
+			if( stopAfter( il, 7 ) ) return WSP_OK;
 		}
+		if( c.decoderStopped() ) return WSP_OK;
 		// final LN + logits = tok_emb^T x (a17): only the last token of each chunk unless all logits were requested
 		kern::SkinnyArgs a = skinny( e.tokEmb, nullptr, hp.n_vocab, d, &e.decLn, nullptr, kern::SK_LOGITS, c.logits );
 		if( !allLogits ) { a.xF32 = c.xd + (size_t)( N - 1 ) * d; a.xStride = (int64_t)N * d; a.nCols = batch; }
@@ -642,7 +655,9 @@ namespace wsp
 	{
 		const Engine& e = *c.e;
 		const int d = e.hp.n_text_state;
-		const bool step = N == 1 && !allLogits;   // the steady state: embedding + all layers + logits in ONE kernel
+		if( c.decoderStopped() && sample && !allLogits ) return fail( WSP_E_INVALIDARG, "no sampling while a decoder stop is set" );
+		// the steady state: embedding + all layers + logits in ONE kernel (a stopped pass runs kernel by kernel)
+		const bool step = N == 1 && !allLogits && !c.decoderStopped();
 		const kern::DecStepArgs sa = stepArgs( c, batch );
 		int n = 0;
 		if( step && c.stepMode == 2 && kern::flowSupported( d, batch, sa.T, sa.H, sa.nTextCtx, c.refThreads, c.flowGeom ) )
@@ -668,7 +683,7 @@ namespace wsp
 	static int decodeSubmit( Context& c, int N, int batch, bool allLogits, bool sample )
 	{
 		int n = 0;
-		if( N == 1 && !allLogits && sample && c.useGraph && !c.prof.on )
+		if( N == 1 && !allLogits && sample && c.useGraph && !c.prof.on && !c.decoderStopped() )
 		{
 			const StepGraphKey key{ batch, c.encCtx, c.refThreads, c.stepMode, c.stepTiming, c.eotArmed };
 			if( !c.stepGraph || !( c.stepGraphKey == key ) )
@@ -692,7 +707,7 @@ namespace wsp
 		}
 		WSP_CHECK( decodeEnqueue( c, N, batch, allLogits, sample, &n ) );
 		launched( n );
-		if( allLogits )
+		if( allLogits && !c.decoderStopped() )
 		{
 			// probabilities for every row (the oracle keeps logits and probs of all N tokens, whisper.cpp:1855-1859); no sampling
 			WSP_CUDA( kern::softmaxRows( c.logits, c.probs, batch * N, c.e->hp.n_vocab, c.stream ) );

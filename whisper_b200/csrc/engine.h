@@ -208,7 +208,12 @@ namespace wsp
 		int lastLogitRows = 0;
 		int nPastHost = 0;              // host mirror of the device-resident n_past (it advances on the device between graph replays)
 		int debugEncLayers = -1;
-		int refThreads = 4;             // reference CPU thread count whose V^T*P arithmetic the decoder reproduces (1..16)
+		// wsp_debug_set_decoder_stop: every decoder pass runs kernel by kernel and ends after op debugDecOp of layer debugDecLayer
+		// (layer -1: after the embedding), without logits or sampling; (-1, -1) = no stop
+		int debugDecLayer = -1, debugDecOp = -1;
+		bool decoderStopped() const { return debugDecLayer >= 0 || debugDecOp >= 0; }
+		int lastPerOpN = 0;             // tokens per chunk of the last kernel-by-kernel decoder pass: the rows of c.xd, qd, attnD, hD
+		int refThreads = 4;            // reference CPU thread count whose V^T*P arithmetic the decoder reproduces (1..16)
 
 		// tensor maps (built once; M of a launch limits the rows touched)
 		CUtensorMap mapMel, mapConv1Even, mapConv1Odd, mapXn, mapAttn, mapH;
